@@ -98,6 +98,18 @@ template <> struct Vec4<float> {
   }
 };
 
+// V (8, 4 or 1) consecutive elements of T <-> float[V]
+template <typename T, int V> __device__ __forceinline__ void load_vec(const T* p, float* f) {
+  if constexpr (V == 8) Vec8<T>::load(p, f);
+  else if constexpr (V == 4) Vec4<T>::load(p, f);
+  else f[0] = to_f(*p);
+}
+template <typename T, int V> __device__ __forceinline__ void store_vec(T* p, const float* f) {
+  if constexpr (V == 8) Vec8<T>::store(p, f);
+  else if constexpr (V == 4) Vec4<T>::store(p, f);
+  else *p = from_f<T>(f[0]);
+}
+
 __device__ __forceinline__ float silu_f(float x) { return x / (1.0f + expf(-x)); }
 // bf16-storage paths: 2-ulp intrinsics are far below the 2^-9 output rounding
 __device__ __forceinline__ float silu_fast(float x) { return __fdividef(x, 1.0f + __expf(-x)); }

@@ -3,6 +3,8 @@
 // fp64 across CTAs so that E[x^2]-E[x]^2 does not cancel.
 #include <stdlib.h>
 
+#include <type_traits>
+
 #include "common.cuh"
 
 // FYC_ZIGZAG (default 1): the norm kernels walk their input back to front.  Activations at the 64x64 level are 84 MB, the L2 is 50
@@ -26,23 +28,23 @@ static int fyc_gn_waves() {
 }
 
 namespace {
-// fp32 pairs: the norm kernels process two lanes' worth of elements per helper call (Hopper has no packed fp32 FMA, so each pair
-// is two scalar instructions with the same round-to-nearest results).
-struct f32x2 { float lo, hi; };
-__device__ __forceinline__ f32x2 pk2(float lo, float hi) { return f32x2{lo, hi}; }
-__device__ __forceinline__ void upk2(f32x2 p, float& lo, float& hi) { lo = p.lo; hi = p.hi; }
-__device__ __forceinline__ f32x2 fma2(f32x2 a, f32x2 b, f32x2 c) { return f32x2{__fmaf_rn(a.lo, b.lo, c.lo), __fmaf_rn(a.hi, b.hi, c.hi)}; }
-__device__ __forceinline__ f32x2 add2(f32x2 a, f32x2 b) { return f32x2{__fadd_rn(a.lo, b.lo), __fadd_rn(a.hi, b.hi)}; }
-__device__ __forceinline__ f32x2 mul2(f32x2 a, f32x2 b) { return f32x2{__fmul_rn(a.lo, b.lo), __fmul_rn(a.hi, b.hi)}; }
-// one 32-bit word holding two bf16 -> packed fp32 pair (element 0 in the low half)
-__device__ __forceinline__ f32x2 bf2_to_f2(uint32_t w) { return pk2(__uint_as_float(w << 16), __uint_as_float(w & 0xffff0000u)); }
-__device__ __forceinline__ uint32_t f2_to_bf2(f32x2 p) {
-  float lo, hi; upk2(p, lo, hi);
+// one 32-bit word holding two bf16 <-> two floats (element 0 in the low half); a 16-byte vector of eight <-> float[8]
+__device__ __forceinline__ void bf2_to_f2(uint32_t w, float& lo, float& hi) { lo = __uint_as_float(w << 16); hi = __uint_as_float(w & 0xffff0000u); }
+__device__ __forceinline__ uint32_t f2_to_bf2(float lo, float hi) {
   __nv_bfloat162 h = __floats2bfloat162_rn(lo, hi);
   return *reinterpret_cast<uint32_t*>(&h);
 }
-__device__ __forceinline__ float ex2_fast(float x) { float y; asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x)); return y; }
-__device__ __forceinline__ float rcp_fast(float x) { float y; asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x)); return y; }
+__device__ __forceinline__ void bf8_to_f(const uint4& raw, float* f) {
+  bf2_to_f2(raw.x, f[0], f[1]); bf2_to_f2(raw.y, f[2], f[3]); bf2_to_f2(raw.z, f[4], f[5]); bf2_to_f2(raw.w, f[6], f[7]);
+}
+__device__ __forceinline__ uint4 f_to_bf8(const float* f) {
+  return make_uint4(f2_to_bf2(f[0], f[1]), f2_to_bf2(f[2], f[3]), f2_to_bf2(f[4], f[5]), f2_to_bf2(f[6], f[7]));
+}
+// four fp32 parameters with one 16-byte load (scalar parameter loads saturated the LSU queue: lg_throttle)
+__device__ __forceinline__ void ldg4(const float* p, float* f) {
+  const float4 a = __ldg(reinterpret_cast<const float4*>(p));
+  f[0] = a.x; f[1] = a.y; f[2] = a.z; f[3] = a.w;
+}
 }  // namespace
 
 // ---------------------------------------------------------------------------------------------------------
@@ -78,34 +80,25 @@ __global__ void __launch_bounds__(256, 4) gn_stats_kernel(const T* __restrict__ 
       for (int e = 0; e < V; ++e) { s[e] = 0.f; q[e] = 0.f; }
       int64_t r = r0 + ry;
       if constexpr (sizeof(T) == 2 && V == 8) {
-        // bf16: 8 independent 16-byte loads in flight per thread, kept packed until they are summed (the 4-deep version was
+        // bf16: 8 independent 16-byte loads in flight per thread, kept as bf16 until they are summed (the 4-deep version was
         // latency-bound: long-scoreboard stalls)
         for (; r + 7 * RY < r1; r += 8 * RY) {
           uint4 raw[8];
 #pragma unroll
           for (int u = 0; u < 8; ++u) raw[u] = __ldg(reinterpret_cast<const uint4*>(base0 + (r + (int64_t)u * RY) * ldx));
-          f32x2 sp[4], qp[4];
-#pragma unroll
-          for (int e = 0; e < 4; ++e) { sp[e] = pk2(s[2 * e], s[2 * e + 1]); qp[e] = pk2(q[2 * e], q[2 * e + 1]); }
 #pragma unroll
           for (int u = 0; u < 8; ++u) {
-            const uint32_t w[4] = {raw[u].x, raw[u].y, raw[u].z, raw[u].w};
+            float f[8];
+            bf8_to_f(raw[u], f);
 #pragma unroll
-            for (int e = 0; e < 4; ++e) { const f32x2 v2 = bf2_to_f2(w[e]); sp[e] = add2(sp[e], v2); qp[e] = fma2(v2, v2, qp[e]); }
+            for (int e = 0; e < 8; ++e) { s[e] = __fadd_rn(s[e], f[e]); q[e] = __fmaf_rn(f[e], f[e], q[e]); }
           }
-#pragma unroll
-          for (int e = 0; e < 4; ++e) { upk2(sp[e], s[2 * e], s[2 * e + 1]); upk2(qp[e], q[2 * e], q[2 * e + 1]); }
         }
       }
       for (; r + 3 * RY < r1; r += 4 * RY) {      // 4 independent 16-byte loads in flight per thread
         float f[4][8];
 #pragma unroll
-        for (int u = 0; u < 4; ++u) {
-          const T* src = base0 + (r + (int64_t)u * RY) * ldx;
-          if constexpr (V == 8) Vec8<T>::load(src, f[u]);
-          else if constexpr (V == 4) Vec4<T>::load(src, f[u]);
-          else f[u][0] = to_f(*src);
-        }
+        for (int u = 0; u < 4; ++u) load_vec<T, V>(base0 + (r + (int64_t)u * RY) * ldx, f[u]);
 #pragma unroll
         for (int u = 0; u < 4; ++u)
 #pragma unroll
@@ -113,9 +106,7 @@ __global__ void __launch_bounds__(256, 4) gn_stats_kernel(const T* __restrict__ 
       }
       for (; r < r1; r += RY) {
         float f[8];
-        if constexpr (V == 8) Vec8<T>::load(base0 + r * ldx, f);
-        else if constexpr (V == 4) Vec4<T>::load(base0 + r * ldx, f);
-        else f[0] = to_f(base0[r * ldx]);
+        load_vec<T, V>(base0 + r * ldx, f);
 #pragma unroll
         for (int e = 0; e < V; ++e) { s[e] += f[e]; q[e] = fmaf(f[e], f[e], q[e]); }
       }
@@ -196,9 +187,7 @@ __global__ void __launch_bounds__(256) gn_apply_kernel(const T* __restrict__ x, 
           const int64_t rw = i / cvn; const int c = (int)(i - rw * cvn) * V;
           src = c < C1 ? x + rw * C1 + c : x2 + rw * (C - C1) + (c - C1);
         }
-        if constexpr (V == 8) Vec8<T>::load(src, f[u]);
-        else if constexpr (V == 4) Vec4<T>::load(src, f[u]);
-        else f[u][0] = to_f(*src);
+        load_vec<T, V>(src, f[u]);
       }
     }
 #pragma unroll
@@ -209,14 +198,9 @@ __global__ void __launch_bounds__(256) gn_apply_kernel(const T* __restrict__ x, 
         const float* sc = scale + nb * C + cv * V;
         const float* sh = shift + nb * C + cv * V;
         float scv[V], shv[V];
-        if constexpr (V >= 4) {     // 16-byte parameter loads (scalar loads saturated the LSU queue: lg_throttle)
+        if constexpr (V >= 4) {
 #pragma unroll
-          for (int e = 0; e < V; e += 4) {
-            float4 a = __ldg(reinterpret_cast<const float4*>(sc + e));
-            float4 b = __ldg(reinterpret_cast<const float4*>(sh + e));
-            scv[e] = a.x; scv[e + 1] = a.y; scv[e + 2] = a.z; scv[e + 3] = a.w;
-            shv[e] = b.x; shv[e + 1] = b.y; shv[e + 2] = b.z; shv[e + 3] = b.w;
-          }
+          for (int e = 0; e < V; e += 4) { ldg4(sc + e, scv + e); ldg4(sh + e, shv + e); }
         } else {
           scv[0] = __ldg(sc); shv[0] = __ldg(sh);
         }
@@ -225,9 +209,7 @@ __global__ void __launch_bounds__(256) gn_apply_kernel(const T* __restrict__ x, 
           float y = fmaf(f[u][e], scv[e], shv[e]);
           f[u][e] = SILU ? (sizeof(T) == 2 ? silu_fast(y) : silu_f(y)) : y;
         }
-        if constexpr (V == 8) Vec8<T>::store(out + i * V, f[u]);
-        else if constexpr (V == 4) Vec4<T>::store(out + i * V, f[u]);
-        else out[i] = from_f<T>(f[u][0]);
+        store_vec<T, V>(out + i * V, f[u]);
       }
       cv += dcv; row += drow;
       if (cv >= cvn) { cv -= cvn; ++row; }
@@ -236,7 +218,7 @@ __global__ void __launch_bounds__(256) gn_apply_kernel(const T* __restrict__ x, 
 }
 
 // bf16 apply, second form: a thread owns ONE 8-channel vector (scale / shift live in 16 registers, loaded once) and walks rows,
-// U rows in flight; the math is packed fp32x2.  The grid-stride form above re-derived (image, channel) and re-loaded four
+// U rows in flight.  The grid-stride form above re-derived (image, channel) and re-loaded four
 // parameter vectors for every 16 bytes of data: 160 issued instructions per vector, 51 us for an 84 MB tensor.
 // [r2] Row blocks (RY x U consecutive rows) are dealt to the CTAs round-robin - neighbouring CTAs stream neighbouring memory at the same
 // time instead of 1184 far-apart private chunks - and the NEXT block's loads are issued before the current block's SiLU math (register
@@ -247,7 +229,7 @@ __device__ __forceinline__ float tanh_fast(float x) { float y; asm("tanh.approx.
 template <bool SILU>
 __global__ void __launch_bounds__(256, 3) gn_apply_rows_kernel(const bf16* __restrict__ x, const float* __restrict__ scale,
                                                             const float* __restrict__ shift, bf16* __restrict__ out, int64_t R,
-                                                            int C, int64_t rows_per_cta, const bf16* __restrict__ x2, int C1) {
+                                                            int C, const bf16* __restrict__ x2, int C1) {
   constexpr int U = 4;
   const int cvn = C / 8;
   const int TX = cvn < 256 ? cvn : 256;
@@ -257,20 +239,14 @@ __global__ void __launch_bounds__(256, 3) gn_apply_rows_kernel(const bf16* __res
   const int64_t nb = blockIdx.y;
   const int64_t blk_rows = (int64_t)RY * U;                     // rows one CTA iteration covers
   const int64_t nblk = (R + blk_rows - 1) / blk_rows;
-  (void)rows_per_cta;
   bf16* ob = out + nb * R * C;
   for (int cv = tx; cv < cvn; cv += TX) {
     const bool second = x2 != nullptr && cv * 8 >= C1;
     const int ldx = x2 == nullptr ? C : (second ? C - C1 : C1);
     const bf16* xb = second ? x2 + nb * R * ldx + (cv * 8 - C1) : x + nb * R * ldx + cv * 8;     // row r of this channel vector: xb + r * ldx
-    f32x2 sc[4], sh[4];
-    {
-      const float4 a0 = __ldg(reinterpret_cast<const float4*>(scale + nb * C + cv * 8)), a1 = __ldg(reinterpret_cast<const float4*>(scale + nb * C + cv * 8 + 4));
-      const float4 b0 = __ldg(reinterpret_cast<const float4*>(shift + nb * C + cv * 8)), b1 = __ldg(reinterpret_cast<const float4*>(shift + nb * C + cv * 8 + 4));
-      sc[0] = pk2(a0.x, a0.y); sc[1] = pk2(a0.z, a0.w); sc[2] = pk2(a1.x, a1.y); sc[3] = pk2(a1.z, a1.w);
-      sh[0] = pk2(b0.x, b0.y); sh[1] = pk2(b0.z, b0.w); sh[2] = pk2(b1.x, b1.y); sh[3] = pk2(b1.z, b1.w);
-    }
-    const f32x2 half2 = pk2(0.5f, 0.5f);
+    float sc[8], sh[8];
+    ldg4(scale + nb * C + cv * 8, sc); ldg4(scale + nb * C + cv * 8 + 4, sc + 4);
+    ldg4(shift + nb * C + cv * 8, sh); ldg4(shift + nb * C + cv * 8 + 4, sh + 4);
     auto load_blk = [&](int64_t blk, uint4* raw) {
 #pragma unroll
       for (int u = 0; u < U; ++u) {
@@ -292,12 +268,14 @@ __global__ void __launch_bounds__(256, 3) gn_apply_rows_kernel(const bf16* __res
         uint32_t o[4];
 #pragma unroll
         for (int e = 0; e < 4; ++e) {
-          f32x2 y = fma2(bf2_to_f2(w[e]), sc[e], sh[e]);
+          float y0, y1;
+          bf2_to_f2(w[e], y0, y1);
+          y0 = __fmaf_rn(y0, sc[2 * e], sh[2 * e]); y1 = __fmaf_rn(y1, sc[2 * e + 1], sh[2 * e + 1]);
           if (SILU) {                       // y * sigmoid(y) = y * (0.5 + 0.5 tanh(y / 2))
-            float h0, h1; upk2(mul2(y, half2), h0, h1);
-            y = mul2(y, fma2(pk2(tanh_fast(h0), tanh_fast(h1)), half2, half2));
+            const float h0 = __fmul_rn(y0, 0.5f), h1 = __fmul_rn(y1, 0.5f);
+            y0 = __fmul_rn(y0, __fmaf_rn(tanh_fast(h0), 0.5f, 0.5f)); y1 = __fmul_rn(y1, __fmaf_rn(tanh_fast(h1), 0.5f, 0.5f));
           }
-          o[e] = f2_to_bf2(y);
+          o[e] = f2_to_bf2(y0, y1);
         }
         *reinterpret_cast<uint4*>(ob + rr * C + cv * 8) = make_uint4(o[0], o[1], o[2], o[3]);
       }
@@ -344,10 +322,9 @@ static int32_t groupnorm_impl(const T* x, const float* gamma, const float* beta,
     int64_t want = ceil_div64((int64_t)fyc_sm_count() * 3, NB);
     const int64_t nblk = ceil_div64(R, (int64_t)RY * 4);
     if (want > nblk) want = nblk;
-    const int64_t rpc = 0;
     dim3 ga((unsigned)want, (unsigned)NB);
-    if (silu) gn_apply_rows_kernel<true><<<ga, 256, 0, st>>>((const bf16*)x, scale, shift, (bf16*)out, R, C, rpc, (const bf16*)x2, C1);
-    else gn_apply_rows_kernel<false><<<ga, 256, 0, st>>>((const bf16*)x, scale, shift, (bf16*)out, R, C, rpc, (const bf16*)x2, C1);
+    if (silu) gn_apply_rows_kernel<true><<<ga, 256, 0, st>>>((const bf16*)x, scale, shift, (bf16*)out, R, C, (const bf16*)x2, C1);
+    else gn_apply_rows_kernel<false><<<ga, 256, 0, st>>>((const bf16*)x, scale, shift, (bf16*)out, R, C, (const bf16*)x2, C1);
     FYC_LAUNCH_CHECK();
     return FYC_OK;
   }
@@ -361,12 +338,18 @@ static int32_t groupnorm_impl(const T* x, const float* gamma, const float* beta,
   return FYC_OK;
 }
 
+// the argument checks fyc_groupnorm and fyc_groupnorm_concat share (C: all normalised channels)
+static int32_t gn_check_args(const char* who, int64_t NB, int64_t R, int64_t C, int64_t G, const void* workspace, size_t workspace_bytes) {
+  FYC_CHECK(G > 0 && C % G == 0, "%s: C=%lld not divisible by G=%lld", who, (long long)C, (long long)G);
+  FYC_CHECK(workspace && workspace_bytes >= fyc_groupnorm_workspace_bytes(NB, C, G), "%s: workspace too small", who);
+  FYC_CHECK(NB > 0 && NB < 65536 && R > 0 && C < (1 << 20) && NB * R < (1ll << 31), "%s: bad shape", who);
+  return FYC_OK;
+}
+
 extern "C" int32_t fyc_groupnorm(const void* x, const float* gamma, const float* beta, void* out, int64_t NB, int64_t R,
                                  int64_t C, int64_t G, float eps, int32_t silu, int32_t dtype, void* workspace,
                                  size_t workspace_bytes, void* stream) {
-  FYC_CHECK(G > 0 && C % G == 0, "groupnorm: C=%lld not divisible by G=%lld", (long long)C, (long long)G);
-  FYC_CHECK(workspace && workspace_bytes >= fyc_groupnorm_workspace_bytes(NB, C, G), "groupnorm: workspace too small");
-  FYC_CHECK(NB > 0 && NB < 65536 && R > 0 && C < (1 << 20) && NB * R < (1ll << 31), "groupnorm: bad shape");
+  if (const int32_t err = gn_check_args("groupnorm", NB, R, C, G, workspace, workspace_bytes)) return err;
   cudaStream_t st = (cudaStream_t)stream;
   if (dtype == FYC_BF16) {
     if (C % 8 == 0) return groupnorm_impl<bf16, 8>((const bf16*)x, gamma, beta, (bf16*)out, NB, R, (int)C, (int)G, eps, silu, workspace, st);
@@ -383,9 +366,7 @@ extern "C" int32_t fyc_groupnorm_concat(const void* x1, int64_t C1, const void* 
                                         void* workspace, size_t workspace_bytes, void* stream) {
   const int64_t C = C1 + C2;
   FYC_CHECK(x1 && x2 && C1 > 0 && C2 > 0, "groupnorm_concat: bad arguments");
-  FYC_CHECK(G > 0 && C % G == 0, "groupnorm_concat: C=%lld not divisible by G=%lld", (long long)C, (long long)G);
-  FYC_CHECK(workspace && workspace_bytes >= fyc_groupnorm_workspace_bytes(NB, C, G), "groupnorm_concat: workspace too small");
-  FYC_CHECK(NB > 0 && NB < 65536 && R > 0 && C < (1 << 20) && NB * R < (1ll << 31), "groupnorm_concat: bad shape");
+  if (const int32_t err = gn_check_args("groupnorm_concat", NB, R, C, G, workspace, workspace_bytes)) return err;
   cudaStream_t st = (cudaStream_t)stream;
   if (dtype == FYC_BF16) {
     FYC_CHECK(C1 % 8 == 0 && C2 % 8 == 0 && ((((uintptr_t)x1 | (uintptr_t)x2 | (uintptr_t)out)) & 15) == 0, "groupnorm_concat(bf16): channel counts must be multiples of 8, pointers 16-byte aligned");
@@ -398,7 +379,66 @@ extern "C" int32_t fyc_groupnorm_concat(const void* x1, int64_t C1, const void* 
 }
 
 // ---------------------------------------------------------------------------------------------------------
-// LayerNorm: one warp per row, row held in registers (two-pass mean / centred variance), optional PE add.
+// LayerNorm.  fyc_layernorm_stats must produce exactly the rstd fyc_layernorm would have used (the LN-folded GEMM replaces the
+// normalised copy by that rstd), so each normalising kernel shares its row statistics with its statistics-only twin.
+
+// warp-per-row form (layernorm_kernel, ln_stats_kernel): loads row xr into registers - lane `lane` holds the channel vectors
+// lane + 32 i below cvn = C / V - and returns its two-pass mean / centred variance
+template <typename T, int V, int NV>
+__device__ __forceinline__ void ln_warp_row_stats(const T* xr, int lane, int cvn, int C, float eps, float (&v)[NV][V], float& mean, float& rstd) {
+  float sum = 0.f;
+#pragma unroll
+  for (int i = 0; i < NV; ++i) {
+    const int cv = lane + 32 * i;
+    if (cv < cvn) {
+      load_vec<T, V>(xr + cv * V, v[i]);
+#pragma unroll
+      for (int e = 0; e < V; ++e) sum += v[i][e];
+    }
+  }
+  mean = warp_sum(sum) / (float)C;
+  float sq = 0.f;
+#pragma unroll
+  for (int i = 0; i < NV; ++i)
+    if (lane + 32 * i < cvn) {
+#pragma unroll
+      for (int e = 0; e < V; ++e) { const float d = v[i][e] - mean; sq = fmaf(d, d, sq); }
+    }
+  rstd = rsqrtf(warp_sum(sq) / (float)C + eps);
+}
+
+// LPR form (layernorm_lpr_kernel, ln_stats_lpr_kernel): LPR lanes share a row of C = 40 * LPR channels, five 16-byte vectors per
+// lane.  From a lane's raw vectors to the centred values v, the row's mean and rstd: two-pass, even and odd elements accumulated
+// separately, combined over the row's lanes by xor-shuffle - every lane of the warp must take part.
+template <int LPR>
+__device__ __forceinline__ void ln_lpr_row_stats(const uint4 (&raw)[5], float eps, float (&v)[5][8], float& mean, float& rstd) {
+  const float inv_c = 1.0f / (float)(LPR * 40);
+  float s0 = 0.f, s1 = 0.f;
+#pragma unroll
+  for (int i = 0; i < 5; ++i) {
+    bf8_to_f(raw[i], v[i]);
+#pragma unroll
+    for (int e = 0; e < 8; e += 2) { s0 = __fadd_rn(s0, v[i][e]); s1 = __fadd_rn(s1, v[i][e + 1]); }
+  }
+  float sum = s0 + s1;
+#pragma unroll
+  for (int o = 1; o < LPR; o <<= 1) sum += __shfl_xor_sync(0xffffffffu, sum, o);
+  mean = sum * inv_c;
+  float q0 = 0.f, q1 = 0.f;
+#pragma unroll
+  for (int i = 0; i < 5; ++i)
+#pragma unroll
+    for (int e = 0; e < 8; e += 2) {
+      v[i][e] = __fadd_rn(v[i][e], -mean); v[i][e + 1] = __fadd_rn(v[i][e + 1], -mean);
+      q0 = __fmaf_rn(v[i][e], v[i][e], q0); q1 = __fmaf_rn(v[i][e + 1], v[i][e + 1], q1);
+    }
+  float sq = q0 + q1;
+#pragma unroll
+  for (int o = 1; o < LPR; o <<= 1) sq += __shfl_xor_sync(0xffffffffu, sq, o);
+  rstd = rsqrtf(sq * inv_c + eps);
+}
+
+// one warp per row, row held in registers, optional PE add
 template <typename T, int V, int NV>
 __global__ void __launch_bounds__(256) layernorm_kernel(const T* __restrict__ x, const float* __restrict__ gamma,
                                                         const float* __restrict__ beta, T* __restrict__ out, int64_t M,
@@ -408,29 +448,8 @@ __global__ void __launch_bounds__(256) layernorm_kernel(const T* __restrict__ x,
   const int64_t row = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
   if (row >= M) return;
   const int cvn = C / V;
-  const T* xr = x + row * C;
-  float v[NV][V];
-  float sum = 0.f;
-#pragma unroll
-  for (int i = 0; i < NV; ++i) {
-    int cv = lane + 32 * i;
-    if (cv < cvn) {
-      if constexpr (V == 8) Vec8<T>::load(xr + cv * V, v[i]); else Vec4<T>::load(xr + cv * V, v[i]);
-#pragma unroll
-      for (int e = 0; e < V; ++e) sum += v[i][e];
-    }
-  }
-  const float mean = warp_sum(sum) / (float)C;
-  float sq = 0.f;
-#pragma unroll
-  for (int i = 0; i < NV; ++i) {
-    int cv = lane + 32 * i;
-    if (cv < cvn) {
-#pragma unroll
-      for (int e = 0; e < V; ++e) { float d = v[i][e] - mean; sq = fmaf(d, d, sq); }
-    }
-  }
-  const float rstd = rsqrtf(warp_sum(sq) / (float)C + eps);
+  float v[NV][V], mean, rstd;
+  ln_warp_row_stats<T, V, NV>(x + row * C, lane, cvn, C, eps, v, mean, rstd);
   const float* per = pe ? pe + ((row / rows_per_frame) % frames) * C : nullptr;
   T* orow = out + row * C;
 #pragma unroll
@@ -438,24 +457,19 @@ __global__ void __launch_bounds__(256) layernorm_kernel(const T* __restrict__ x,
     int cv = lane + 32 * i;
     if (cv < cvn) {
       float o[V], gm[V], bt[V];
-      // 16-byte parameter loads (scalar loads here saturated the LSU queue)
 #pragma unroll
-      for (int e = 0; e < V; e += 4) {
-        float4 g4 = __ldg(reinterpret_cast<const float4*>(gamma + cv * V + e));
-        float4 b4 = __ldg(reinterpret_cast<const float4*>(beta + cv * V + e));
-        gm[e] = g4.x; gm[e + 1] = g4.y; gm[e + 2] = g4.z; gm[e + 3] = g4.w;
-        bt[e] = b4.x; bt[e + 1] = b4.y; bt[e + 2] = b4.z; bt[e + 3] = b4.w;
-      }
+      for (int e = 0; e < V; e += 4) { ldg4(gamma + cv * V + e, gm + e); ldg4(beta + cv * V + e, bt + e); }
       if (per) {
 #pragma unroll
         for (int e = 0; e < V; e += 4) {
-          float4 p4 = __ldg(reinterpret_cast<const float4*>(per + cv * V + e));
-          bt[e] += p4.x; bt[e + 1] += p4.y; bt[e + 2] += p4.z; bt[e + 3] += p4.w;
+          float p4[4];
+          ldg4(per + cv * V + e, p4);
+          bt[e] += p4[0]; bt[e + 1] += p4[1]; bt[e + 2] += p4[2]; bt[e + 3] += p4[3];
         }
       }
 #pragma unroll
       for (int e = 0; e < V; ++e) o[e] = (v[i][e] - mean) * rstd * gm[e] + bt[e];
-      if constexpr (V == 8) Vec8<T>::store(orow + cv * V, o); else Vec4<T>::store(orow + cv * V, o);
+      store_vec<T, V>(orow + cv * V, o);
     }
   }
 }
@@ -463,6 +477,7 @@ __global__ void __launch_bounds__(256) layernorm_kernel(const T* __restrict__ x,
 // bf16 LayerNorm, RPW rows per warp: every row's 16-byte vectors are requested before any is used (RPW x NV loads in
 // flight per lane instead of NV), gamma / beta are read once per warp instead of once per row.  The one-row kernel ran at
 // 2.6 TB/s of the 6.6 TB/s the copy benchmark reaches: too few bytes in flight per SM and ~5 parameter loads per data load.
+// (Its statistics multiply by 1 / C where the warp-per-row pair divides by C: it has no statistics-only twin to agree with.)
 template <int NV, int RPW>
 __global__ void __launch_bounds__(256) layernorm_bf16_kernel(const bf16* __restrict__ x, const float* __restrict__ gamma,
                                                              const float* __restrict__ beta, bf16* __restrict__ out, int64_t M,
@@ -487,12 +502,7 @@ __global__ void __launch_bounds__(256) layernorm_bf16_kernel(const bf16* __restr
     const int cv = lane + 32 * i;
     if (cv < cvn) {
 #pragma unroll
-      for (int e = 0; e < 8; e += 4) {
-        const float4 g4 = __ldg(reinterpret_cast<const float4*>(gamma + cv * 8 + e));
-        const float4 b4 = __ldg(reinterpret_cast<const float4*>(beta + cv * 8 + e));
-        gm[i][e] = g4.x; gm[i][e + 1] = g4.y; gm[i][e + 2] = g4.z; gm[i][e + 3] = g4.w;
-        bt[i][e] = b4.x; bt[i][e + 1] = b4.y; bt[i][e + 2] = b4.z; bt[i][e + 3] = b4.w;
-      }
+      for (int e = 0; e < 8; e += 4) { ldg4(gamma + cv * 8 + e, gm[i] + e); ldg4(beta + cv * 8 + e, bt[i] + e); }
     }
   }
   const float inv_c = 1.0f / (float)C;
@@ -504,9 +514,7 @@ __global__ void __launch_bounds__(256) layernorm_bf16_kernel(const bf16* __restr
     float sum = 0.f;
 #pragma unroll
     for (int i = 0; i < NV; ++i) {
-      const uint32_t w[4] = {raw[r][i].x, raw[r][i].y, raw[r][i].z, raw[r][i].w};
-#pragma unroll
-      for (int e = 0; e < 4; ++e) { v[i][2 * e] = __uint_as_float(w[e] << 16); v[i][2 * e + 1] = __uint_as_float(w[e] & 0xffff0000u); }
+      bf8_to_f(raw[r][i], v[i]);
       if (lane + 32 * i < cvn) {
 #pragma unroll
         for (int e = 0; e < 8; ++e) sum += v[i][e];
@@ -527,10 +535,7 @@ __global__ void __launch_bounds__(256) layernorm_bf16_kernel(const bf16* __restr
       const int cv = lane + 32 * i;
       if (cv < cvn) {
         float o[8], pb[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
-        if (per) {
-          const float4 p0 = __ldg(reinterpret_cast<const float4*>(per + cv * 8)), p1 = __ldg(reinterpret_cast<const float4*>(per + cv * 8 + 4));
-          pb[0] = p0.x; pb[1] = p0.y; pb[2] = p0.z; pb[3] = p0.w; pb[4] = p1.x; pb[5] = p1.y; pb[6] = p1.z; pb[7] = p1.w;
-        }
+        if (per) { ldg4(per + cv * 8, pb); ldg4(per + cv * 8 + 4, pb + 4); }
 #pragma unroll
         for (int e = 0; e < 8; ++e) o[e] = (v[i][e] - mean) * rstd * gm[i][e] + (bt[i][e] + pb[e]);
         Vec8<bf16>::store(out + row * C + cv * 8, o);
@@ -541,9 +546,9 @@ __global__ void __launch_bounds__(256) layernorm_bf16_kernel(const bf16* __restr
 
 // bf16 LayerNorm for C = 40 * LPR (320 / 640 / 1280): LPR lanes share a row, five 16-byte vectors per lane - every lane is busy
 // (the warp-per-row kernels idle 24 of 32 lanes on the second vector of a 320-wide row), 32 / LPR rows per warp pass, PASSES passes
-// with all loads of a pass issued up front.  gamma / beta stay in registers for the warp's lifetime; the arithmetic is the same
-// two-pass (mean, then centred variance) as the reference kernel, on packed fp32 pairs: ~5 issued instructions per element
-// instead of ~18.
+// with all loads of a pass issued up front.  gamma stays in registers for the warp's lifetime; the arithmetic is the same
+// two-pass (mean, then centred variance) as the reference kernel in explicitly rounded, never contracted fp32 steps: ~5 issued
+// instructions per element instead of ~18.
 template <int LPR, int PASSES, bool HAS_PE>
 __global__ void __launch_bounds__(256, 2) layernorm_lpr_kernel(const bf16* __restrict__ x, const float* __restrict__ gamma,
                                                                const float* __restrict__ beta, bf16* __restrict__ out, int64_t M,
@@ -557,15 +562,11 @@ __global__ void __launch_bounds__(256, 2) layernorm_lpr_kernel(const bf16* __res
   const int64_t bxl = rev ? (int64_t)gridDim.x - 1 - blockIdx.x : (int64_t)blockIdx.x;
   const int64_t row_base = (bxl * (blockDim.x >> 5) + (threadIdx.x >> 5)) * (RPP * PASSES);
   if (row_base >= M) return;
-  f32x2 gm[5][4];                                       // beta is re-read from L1 per vector: 40 more registers would halve the occupancy
+  float gm[5][8];                                       // beta is re-read from L1 per vector: 40 more registers would halve the occupancy
   const float* gp = gamma + sub * 8;
   const float* bp = beta + sub * 8;
 #pragma unroll
-  for (int i = 0; i < 5; ++i) {
-    const float4 g0 = __ldg(reinterpret_cast<const float4*>(gp + i * VS)), g1 = __ldg(reinterpret_cast<const float4*>(gp + i * VS + 4));
-    gm[i][0] = pk2(g0.x, g0.y); gm[i][1] = pk2(g0.z, g0.w); gm[i][2] = pk2(g1.x, g1.y); gm[i][3] = pk2(g1.z, g1.w);
-  }
-  const float inv_c = 1.0f / (float)C;
+  for (int i = 0; i < 5; ++i) { ldg4(gp + i * VS, gm[i]); ldg4(gp + i * VS + 4, gm[i] + 4); }
 #pragma unroll 1
   for (int ps = 0; ps < PASSES; ++ps) {
     const int64_t row = row_base + ps * RPP + rr;
@@ -575,53 +576,31 @@ __global__ void __launch_bounds__(256, 2) layernorm_lpr_kernel(const bf16* __res
     uint4 raw[5];
 #pragma unroll
     for (int i = 0; i < 5; ++i) raw[i] = __ldg(reinterpret_cast<const uint4*>(xr + i * VS));
-    f32x2 v[5][4];
-    f32x2 s2 = pk2(0.f, 0.f);
-#pragma unroll
-    for (int i = 0; i < 5; ++i) {
-      const uint32_t w[4] = {raw[i].x, raw[i].y, raw[i].z, raw[i].w};
-#pragma unroll
-      for (int e = 0; e < 4; ++e) { v[i][e] = bf2_to_f2(w[e]); s2 = add2(s2, v[i][e]); }
-    }
-    float s0, s1; upk2(s2, s0, s1);
-    float sum = s0 + s1;
-#pragma unroll
-    for (int o = 1; o < LPR; o <<= 1) sum += __shfl_xor_sync(0xffffffffu, sum, o);
-    const float mean = sum * inv_c;
-    const f32x2 nmean = pk2(-mean, -mean);
-    f32x2 q2 = pk2(0.f, 0.f);
-#pragma unroll
-    for (int i = 0; i < 5; ++i)
-#pragma unroll
-      for (int e = 0; e < 4; ++e) { v[i][e] = add2(v[i][e], nmean); q2 = fma2(v[i][e], v[i][e], q2); }
-    float q0, q1; upk2(q2, q0, q1);
-    float sq = q0 + q1;
-#pragma unroll
-    for (int o = 1; o < LPR; o <<= 1) sq += __shfl_xor_sync(0xffffffffu, sq, o);
-    const float rstd = rsqrtf(sq * inv_c + eps);
-    const f32x2 rstd2 = pk2(rstd, rstd);
+    float v[5][8], mean, rstd;
+    ln_lpr_row_stats<LPR>(raw, eps, v, mean, rstd);
     const float* pp = HAS_PE ? pe + ((rowc / rows_per_frame) % frames) * C + sub * 8 : nullptr;
     bf16* orow = out + rowc * C + sub * 8;
 #pragma unroll
     for (int i = 0; i < 5; ++i) {
-      const float4 b0 = __ldg(reinterpret_cast<const float4*>(bp + i * VS)), b1 = __ldg(reinterpret_cast<const float4*>(bp + i * VS + 4));
-      f32x2 bb[4] = {pk2(b0.x, b0.y), pk2(b0.z, b0.w), pk2(b1.x, b1.y), pk2(b1.z, b1.w)};
+      float bb[8], o[8];
+      ldg4(bp + i * VS, bb); ldg4(bp + i * VS + 4, bb + 4);
       if (HAS_PE) {
-        const float4 p0 = __ldg(reinterpret_cast<const float4*>(pp + i * VS)), p1 = __ldg(reinterpret_cast<const float4*>(pp + i * VS + 4));
-        bb[0] = add2(bb[0], pk2(p0.x, p0.y)); bb[1] = add2(bb[1], pk2(p0.z, p0.w));
-        bb[2] = add2(bb[2], pk2(p1.x, p1.y)); bb[3] = add2(bb[3], pk2(p1.z, p1.w));
-      }
-      uint32_t o[4];
+        float pb[8];
+        ldg4(pp + i * VS, pb); ldg4(pp + i * VS + 4, pb + 4);
 #pragma unroll
-      for (int e = 0; e < 4; ++e) o[e] = f2_to_bf2(fma2(mul2(v[i][e], rstd2), gm[i][e], bb[e]));
-      if (ok) *reinterpret_cast<uint4*>(orow + i * VS) = make_uint4(o[0], o[1], o[2], o[3]);
+        for (int e = 0; e < 8; ++e) bb[e] = __fadd_rn(bb[e], pb[e]);
+      }
+#pragma unroll
+      for (int e = 0; e < 8; ++e) o[e] = __fmaf_rn(__fmul_rn(v[i][e], rstd), gm[i][e], bb[e]);
+      const uint4 packed = f_to_bf8(o);
+      if (ok) *reinterpret_cast<uint4*>(orow + i * VS) = packed;
     }
   }
 }
 
 // LayerNorm STATISTICS only (fyc_layernorm_stats): per row rstd (fp32) and the 8-column bf16 "aug" row [m_hi, m_hi, m_lo, m_lo, 0, 0, 0, 0]
 // (mean = m_hi + m_lo) that the LN-folded GEMM appends to its K dimension (fyc.h FYC_EPI_LNFOLD).  Same lane layout and the same
-// two-pass arithmetic as layernorm_lpr_kernel - one read of x, no write of a normalised copy.  PASSES x 5 independent 16-byte loads
+// row statistics as layernorm_lpr_kernel - one read of x, no write of a normalised copy.  PASSES x 5 independent 16-byte loads
 // per lane are requested before the first is used.
 __device__ __forceinline__ void ln_write_stats(float* __restrict__ rstd_out, bf16* __restrict__ aug, int64_t row, float mean, float rstd) {
   rstd_out[row] = rstd;
@@ -640,12 +619,11 @@ __global__ void __launch_bounds__(256, 2) ln_stats_lpr_kernel(const bf16* __rest
   const int64_t bxl = rev ? (int64_t)gridDim.x - 1 - blockIdx.x : (int64_t)blockIdx.x;
   const int64_t row_base = (bxl * (blockDim.x >> 5) + (threadIdx.x >> 5)) * (RPP * PASSES);
   if (row_base >= M) return;
-  const float inv_c = 1.0f / (float)C;
   uint4 raw[PASSES][5];
 #pragma unroll
   for (int ps = 0; ps < PASSES; ++ps) {
     const int64_t row = row_base + ps * RPP + rr;
-    const int64_t rowc = row < M ? row : M - 1;
+    const int64_t rowc = row < M ? row : M - 1;       // out-of-range lanes shadow the last row (shuffles stay full-warp), never store
     const bf16* xr = x + rowc * C + sub * 8;
 #pragma unroll
     for (int i = 0; i < 5; ++i) raw[ps][i] = __ldg(reinterpret_cast<const uint4*>(xr + i * VS));
@@ -653,30 +631,8 @@ __global__ void __launch_bounds__(256, 2) ln_stats_lpr_kernel(const bf16* __rest
 #pragma unroll
   for (int ps = 0; ps < PASSES; ++ps) {
     const int64_t row = row_base + ps * RPP + rr;
-    f32x2 v[5][4];
-    f32x2 s2 = pk2(0.f, 0.f);
-#pragma unroll
-    for (int i = 0; i < 5; ++i) {
-      const uint32_t w[4] = {raw[ps][i].x, raw[ps][i].y, raw[ps][i].z, raw[ps][i].w};
-#pragma unroll
-      for (int e = 0; e < 4; ++e) { v[i][e] = bf2_to_f2(w[e]); s2 = add2(s2, v[i][e]); }
-    }
-    float s0, s1; upk2(s2, s0, s1);
-    float sum = s0 + s1;
-#pragma unroll
-    for (int o = 1; o < LPR; o <<= 1) sum += __shfl_xor_sync(0xffffffffu, sum, o);
-    const float mean = sum * inv_c;
-    const f32x2 nmean = pk2(-mean, -mean);
-    f32x2 q2 = pk2(0.f, 0.f);
-#pragma unroll
-    for (int i = 0; i < 5; ++i)
-#pragma unroll
-      for (int e = 0; e < 4; ++e) { const f32x2 d = add2(v[i][e], nmean); q2 = fma2(d, d, q2); }
-    float q0, q1; upk2(q2, q0, q1);
-    float sq = q0 + q1;
-#pragma unroll
-    for (int o = 1; o < LPR; o <<= 1) sq += __shfl_xor_sync(0xffffffffu, sq, o);
-    const float rstd = rsqrtf(sq * inv_c + eps);
+    float v[5][8], mean, rstd;
+    ln_lpr_row_stats<LPR>(raw[ps], eps, v, mean, rstd);
     if (sub == 0 && row < M) ln_write_stats(rstd_out, aug, row, mean, rstd);
   }
 }
@@ -688,50 +644,51 @@ __global__ void __launch_bounds__(256) ln_stats_kernel(const T* __restrict__ x, 
   const int64_t row = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
   if (row >= M) return;
   const int cvn = C / V;
-  const T* xr = x + row * C;
-  float v[NV][V];
-  float sum = 0.f;
-#pragma unroll
-  for (int i = 0; i < NV; ++i) {
-    const int cv = lane + 32 * i;
-    if (cv < cvn) {
-      if constexpr (V == 8) Vec8<T>::load(xr + cv * V, v[i]); else Vec4<T>::load(xr + cv * V, v[i]);
-#pragma unroll
-      for (int e = 0; e < V; ++e) sum += v[i][e];
-    }
-  }
-  const float mean = warp_sum(sum) / (float)C;
-  float sq = 0.f;
-#pragma unroll
-  for (int i = 0; i < NV; ++i)
-    if (lane + 32 * i < cvn) {
-#pragma unroll
-      for (int e = 0; e < V; ++e) { const float d = v[i][e] - mean; sq = fmaf(d, d, sq); }
-    }
-  const float rstd = rsqrtf(warp_sum(sq) / (float)C + eps);
+  float v[NV][V], mean, rstd;
+  ln_warp_row_stats<T, V, NV>(x + row * C, lane, cvn, C, eps, v, mean, rstd);
   if (lane == 0) ln_write_stats(rstd_out, aug, row, mean, rstd);
+}
+
+// The row-width classes of fyc_layernorm and fyc_layernorm_stats (C already checked: a multiple of V, <= 2048): calls
+// f(LPR, NV) with compile-time constants - LPR != 0: an LPR kernel (bf16, C = 40 * LPR); LPR == 0: a warp-per-row kernel with
+// NV vectors of V = 16 / sizeof(T) elements per lane.
+template <int N> using int_c = std::integral_constant<int, N>;
+template <typename T, typename F>
+static void ln_for_width(int64_t C, F f) {
+  if constexpr (sizeof(T) == 2) {
+    if (C == 320) f(int_c<8>(), int_c<5>());
+    else if (C == 640) f(int_c<16>(), int_c<5>());
+    else if (C == 1280) f(int_c<32>(), int_c<5>());
+    else if (C <= 8 * 32 * 5) f(int_c<0>(), int_c<5>());
+    else f(int_c<0>(), int_c<8>());
+  } else {
+    if (C <= 4 * 32 * 5) f(int_c<0>(), int_c<5>());
+    else if (C <= 4 * 32 * 10) f(int_c<0>(), int_c<10>());
+    else f(int_c<0>(), int_c<16>());
+  }
+}
+
+template <typename T>
+static void layernorm_stats_launch(const T* x, float* rstd, bf16* aug, int64_t M, int64_t C, float eps, cudaStream_t st) {
+  ln_for_width<T>(C, [&](auto lpr, auto nv) {
+    constexpr int LPR = decltype(lpr)::value, NV = decltype(nv)::value, PASSES = 4;
+    if constexpr (LPR != 0)
+      ln_stats_lpr_kernel<LPR, PASSES><<<(unsigned)ceil_div64(M, 8 * (32 / LPR) * PASSES), 256, 0, st>>>(x, rstd, aug, M, eps, fyc_zigzag());
+    else
+      ln_stats_kernel<T, 16 / sizeof(T), NV><<<(unsigned)ceil_div64(M, 8), 256, 0, st>>>(x, rstd, aug, M, (int)C, eps);
+  });
 }
 
 extern "C" int32_t fyc_layernorm_stats(const void* x, float* rstd, void* aug, int64_t M, int64_t C, float eps, int32_t dtype, void* stream) {
   cudaStream_t st = (cudaStream_t)stream;
   FYC_CHECK(x && rstd && M > 0 && C > 0, "layernorm_stats: bad arguments");
   FYC_CHECK((((uintptr_t)x | (uintptr_t)aug) & 15) == 0 && (((uintptr_t)rstd) & 3) == 0, "layernorm_stats: alignment");
-  bf16* ao = (bf16*)aug;
-  const unsigned grid = (unsigned)ceil_div64(M, 8);
   if (dtype == FYC_BF16) {
     FYC_CHECK(C % 8 == 0 && C <= 2048, "layernorm_stats(bf16): C=%lld must be a multiple of 8 and <= 2048", (long long)C);
-    const bf16* xb = (const bf16*)x;
-    constexpr int PASSES = 4;
-    if (C == 320) ln_stats_lpr_kernel<8, PASSES><<<(unsigned)ceil_div64(M, 8 * 4 * PASSES), 256, 0, st>>>(xb, rstd, ao, M, eps, fyc_zigzag());
-    else if (C == 640) ln_stats_lpr_kernel<16, PASSES><<<(unsigned)ceil_div64(M, 8 * 2 * PASSES), 256, 0, st>>>(xb, rstd, ao, M, eps, fyc_zigzag());
-    else if (C == 1280) ln_stats_lpr_kernel<32, PASSES><<<(unsigned)ceil_div64(M, 8 * 1 * PASSES), 256, 0, st>>>(xb, rstd, ao, M, eps, fyc_zigzag());
-    else if (C <= 8 * 32 * 5) ln_stats_kernel<bf16, 8, 5><<<grid, 256, 0, st>>>(xb, rstd, ao, M, (int)C, eps);
-    else ln_stats_kernel<bf16, 8, 8><<<grid, 256, 0, st>>>(xb, rstd, ao, M, (int)C, eps);
+    layernorm_stats_launch((const bf16*)x, rstd, (bf16*)aug, M, C, eps, st);
   } else if (dtype == FYC_F32) {
     FYC_CHECK(C % 4 == 0 && C <= 2048, "layernorm_stats(f32): C=%lld must be a multiple of 4 and <= 2048", (long long)C);
-    if (C <= 4 * 32 * 5) ln_stats_kernel<float, 4, 5><<<grid, 256, 0, st>>>((const float*)x, rstd, ao, M, (int)C, eps);
-    else if (C <= 4 * 32 * 10) ln_stats_kernel<float, 4, 10><<<grid, 256, 0, st>>>((const float*)x, rstd, ao, M, (int)C, eps);
-    else ln_stats_kernel<float, 4, 16><<<grid, 256, 0, st>>>((const float*)x, rstd, ao, M, (int)C, eps);
+    layernorm_stats_launch((const float*)x, rstd, (bf16*)aug, M, C, eps, st);
   } else {
     FYC_CHECK(false, "layernorm_stats: unknown dtype %d", dtype);
   }
@@ -739,13 +696,23 @@ extern "C" int32_t fyc_layernorm_stats(const void* x, float* rstd, void* aug, in
   return FYC_OK;
 }
 
-template <int LPR>
-static void launch_ln_lpr(const bf16* xb, const float* gamma, const float* beta, bf16* ob, int64_t M, float eps, const float* pe,
-                          int64_t rows_per_frame, int64_t frames, cudaStream_t st) {
-  constexpr int PASSES = 2;
-  const unsigned grid = (unsigned)ceil_div64(M, 8 * (32 / LPR) * PASSES);
-  if (pe) layernorm_lpr_kernel<LPR, PASSES, true><<<grid, 256, 0, st>>>(xb, gamma, beta, ob, M, eps, pe, rows_per_frame, frames, fyc_zigzag());
-  else layernorm_lpr_kernel<LPR, PASSES, false><<<grid, 256, 0, st>>>(xb, gamma, beta, ob, M, eps, pe, rows_per_frame, frames, fyc_zigzag());
+template <typename T>
+static void layernorm_launch(const T* x, const float* gamma, const float* beta, T* out, int64_t M, int64_t C, float eps, const float* pe,
+                             int64_t rows_per_frame, int64_t frames, cudaStream_t st) {
+  ln_for_width<T>(C, [&](auto lpr, auto nv) {
+    constexpr int LPR = decltype(lpr)::value, NV = decltype(nv)::value, PASSES = 2;
+    if constexpr (LPR != 0) {
+      const unsigned grid = (unsigned)ceil_div64(M, 8 * (32 / LPR) * PASSES);
+      if (pe) layernorm_lpr_kernel<LPR, PASSES, true><<<grid, 256, 0, st>>>(x, gamma, beta, out, M, eps, pe, rows_per_frame, frames, fyc_zigzag());
+      else layernorm_lpr_kernel<LPR, PASSES, false><<<grid, 256, 0, st>>>(x, gamma, beta, out, M, eps, pe, rows_per_frame, frames, fyc_zigzag());
+    } else {
+      if constexpr (sizeof(T) == 2) {       // narrow bf16 rows: several rows per warp
+        if (C <= 8 * 32 * 2) return layernorm_bf16_kernel<2, 4><<<(unsigned)ceil_div64(M, 8 * 4), 256, 0, st>>>(x, gamma, beta, out, M, (int)C, eps, pe, rows_per_frame, frames);
+        if (C <= 8 * 32 * 3) return layernorm_bf16_kernel<3, 2><<<(unsigned)ceil_div64(M, 8 * 2), 256, 0, st>>>(x, gamma, beta, out, M, (int)C, eps, pe, rows_per_frame, frames);
+      }
+      layernorm_kernel<T, 16 / sizeof(T), NV><<<(unsigned)ceil_div64(M, 8), 256, 0, st>>>(x, gamma, beta, out, M, (int)C, eps, pe, rows_per_frame, frames);
+    }
+  });
 }
 
 extern "C" int32_t fyc_layernorm(const void* x, const float* gamma, const float* beta, void* out, int64_t M, int64_t C,
@@ -754,23 +721,13 @@ extern "C" int32_t fyc_layernorm(const void* x, const float* gamma, const float*
   cudaStream_t st = (cudaStream_t)stream;
   FYC_CHECK(M > 0 && C > 0, "layernorm: bad shape");
   if (pe) FYC_CHECK(rows_per_frame > 0 && frames > 0, "layernorm: pe needs rows_per_frame/frames");
-  unsigned grid = (unsigned)ceil_div64(M, 8);
   if (dtype == FYC_BF16) {
     FYC_CHECK(C % 8 == 0 && C <= 8 * 32 * 8, "layernorm(bf16): C=%lld must be a multiple of 8 and <= 2048", (long long)C);
     FYC_CHECK((((uintptr_t)x | (uintptr_t)out) & 15) == 0 && (((uintptr_t)gamma | (uintptr_t)beta | (uintptr_t)pe) & 15) == 0, "layernorm(bf16): 16-byte alignment");
-    const bf16* xb = (const bf16*)x; bf16* ob = (bf16*)out;
-    if (C == 320) launch_ln_lpr<8>(xb, gamma, beta, ob, M, eps, pe, rows_per_frame, frames, st);
-    else if (C == 640) launch_ln_lpr<16>(xb, gamma, beta, ob, M, eps, pe, rows_per_frame, frames, st);
-    else if (C == 1280) launch_ln_lpr<32>(xb, gamma, beta, ob, M, eps, pe, rows_per_frame, frames, st);
-    else if (C <= 8 * 32 * 2) layernorm_bf16_kernel<2, 4><<<(unsigned)ceil_div64(M, 8 * 4), 256, 0, st>>>(xb, gamma, beta, ob, M, (int)C, eps, pe, rows_per_frame, frames);
-    else if (C <= 8 * 32 * 3) layernorm_bf16_kernel<3, 2><<<(unsigned)ceil_div64(M, 8 * 2), 256, 0, st>>>(xb, gamma, beta, ob, M, (int)C, eps, pe, rows_per_frame, frames);
-    else if (C <= 8 * 32 * 5) layernorm_kernel<bf16, 8, 5><<<grid, 256, 0, st>>>(xb, gamma, beta, ob, M, (int)C, eps, pe, rows_per_frame, frames);
-    else layernorm_kernel<bf16, 8, 8><<<grid, 256, 0, st>>>(xb, gamma, beta, ob, M, (int)C, eps, pe, rows_per_frame, frames);
+    layernorm_launch((const bf16*)x, gamma, beta, (bf16*)out, M, C, eps, pe, rows_per_frame, frames, st);
   } else if (dtype == FYC_F32) {
     FYC_CHECK(C % 4 == 0 && C <= 4 * 32 * 16, "layernorm(f32): C=%lld must be a multiple of 4 and <= 2048", (long long)C);
-    if (C <= 4 * 32 * 5) layernorm_kernel<float, 4, 5><<<grid, 256, 0, st>>>((const float*)x, gamma, beta, (float*)out, M, (int)C, eps, pe, rows_per_frame, frames);
-    else if (C <= 4 * 32 * 10) layernorm_kernel<float, 4, 10><<<grid, 256, 0, st>>>((const float*)x, gamma, beta, (float*)out, M, (int)C, eps, pe, rows_per_frame, frames);
-    else layernorm_kernel<float, 4, 16><<<grid, 256, 0, st>>>((const float*)x, gamma, beta, (float*)out, M, (int)C, eps, pe, rows_per_frame, frames);
+    layernorm_launch((const float*)x, gamma, beta, (float*)out, M, C, eps, pe, rows_per_frame, frames, st);
   } else {
     FYC_CHECK(false, "layernorm: unknown dtype %d", dtype);
   }

@@ -360,6 +360,36 @@ class UNet3DConditionModel(ParamTreeModel):
             return wp, cb.contiguous(), rb
         return self._cached(("lnfold", name), make)
 
+    def _ln_proj(self, tok, norm, name, fold_w, plain, fold_bias=None, ok=True, geglu=False, pe=None, clips=0, frames=0, rows_per_frame=0):
+        """LayerNorm `norm` of the tokens [M, C] followed by a projection.  Where the fold applies (ops.ln_fold_ok and the site's own
+        condition ``ok``) the norm lives in the GEMM: one read-only statistics pass + epilogue terms (_ln_fold, cache key ``name``, built
+        from the unrounded fp32 thunks ``fold_w`` / ``fold_bias``) instead of writing and re-reading a normalised copy.  Otherwise
+        ops.layernorm and a plain GEMM on ``plain()`` = (packed weight, bias or None).  ``pe``: temporal position table added after the
+        norm, row r belongs to frame (r // rows_per_frame) % frames of one of ``clips`` clips."""
+        M, C = tok.shape
+        if ops.ln_fold_ok(tok.dtype, M, C) and ok:
+            w, cb, rbt = self._ln_fold(name, norm, fold_w, fold_bias, interleave=geglu, pe=pe)
+            rb = None
+            if pe is not None:      # (LN(x) + pe_f) W^T = LN-folded GEMM + the per-frame row-bias table pe W^T; row group = (clip, frame)
+                rb = self._cached(("pe_rb", name, clips, frames), lambda: rbt[:frames].repeat(clips, 1).contiguous())
+            return ops.gemm(tok, w, bias=cb, rowbias=rb, rows_per_group=rows_per_frame if pe is not None else 0, geglu=geglu,
+                            ln=ops.layernorm_stats(tok))
+        n = ops.layernorm(tok, self._f(norm + ".weight"), self._f(norm + ".bias"), pe=pe, rows_per_frame=rows_per_frame, frames=frames)
+        w, b = plain()
+        return ops.gemm(n, w, bias=b, geglu=geglu)
+
+    @staticmethod
+    def _gemm_replicas(A, rep, W, **kw):
+        """``rep`` row blocks of A, each through the same GEMM (weight, bias, residual / second source shared by all of them: the CFG
+        replicas over one copy of what they have in common) -> [rep * rows, N].  One replica is the plain un-sliced call."""
+        if rep == 1:
+            return ops.gemm(A, W, **kw)
+        rows = A.shape[0] // rep
+        out = torch.empty((A.shape[0], W.shape[0]), dtype=A.dtype, device=A.device)
+        for r in range(rep):
+            ops.gemm(A[r * rows:(r + 1) * rows], W, out=out[r * rows:(r + 1) * rows], **kw)
+        return out
+
     def _freqs(self):
         def make():
             half = self._cfg["block_out_channels"][0] // 2
@@ -412,13 +442,7 @@ class UNet3DConditionModel(ParamTreeModel):
         h = self._gn(p + ".norm2", h, B, True, False)
         if self._has(p + ".conv_shortcut.weight"):
             w_s, b_s = self._w1x1(p + ".conv_shortcut.weight"), self._f(p + ".conv_shortcut.bias")
-            if rep == 1:
-                res = ops.gemm(x.view(-1, Cin), w_s, bias=b_s, A2=None if skip is None else skip.view(-1, skip.shape[-1]))
-            else:
-                rows = (NB // rep) * H * W
-                res = torch.empty((NB * H * W, w_s.shape[0]), dtype=x.dtype, device=x.device)
-                for r in range(rep):
-                    ops.gemm(x.view(-1, Cin)[r * rows:(r + 1) * rows], w_s, bias=b_s, A2=skip.view(-1, skip.shape[-1]), out=res[r * rows:(r + 1) * rows])
+            res = self._gemm_replicas(x.view(-1, Cin), rep, w_s, bias=b_s, A2=None if skip is None else skip.view(-1, skip.shape[-1]))
             res = res.view(NB, H, W, -1)
         else:
             res = x if skip is None else ops.concat_channels(x, skip if rep == 1 else skip.repeat(rep, 1, 1, 1))
@@ -427,15 +451,9 @@ class UNet3DConditionModel(ParamTreeModel):
     def _ff(self, p, tok, norm):
         """x + W2 (a . gelu(g)),  [a, g] = W1 LN(x) + b1  (attention.py:563, motion_module.py:282): LayerNorm `norm` folded into the GEGLU GEMM
         in tensor-core mode"""
-        M, C = tok.shape
-        if ops.ln_fold_ok(tok.dtype, M, C) and C % 32 == 0:          # 8 C rows in 256-row GEGLU tiles
-            w1, cb, _ = self._ln_fold(p + ".net.0.proj", norm, lambda: self._p(p + ".net.0.proj.weight").detach(),
-                                      lambda: self._p(p + ".net.0.proj.bias").detach(), interleave=True)
-            h = ops.gemm(tok, w1, bias=cb, geglu=True, ln=ops.layernorm_stats(tok))
-        else:
-            n = ops.layernorm(tok, self._f(norm + ".weight"), self._f(norm + ".bias"))
-            w1, b1 = self._geglu(p)
-            h = ops.gemm(n, w1, bias=b1, geglu=True)
+        h = self._ln_proj(tok, norm, p + ".net.0.proj", lambda: self._p(p + ".net.0.proj.weight").detach(), lambda: self._geglu(p),
+                          fold_bias=lambda: self._p(p + ".net.0.proj.bias").detach(), geglu=True,
+                          ok=tok.shape[1] % 32 == 0)                 # 8 C rows in 256-row GEGLU tiles
         return ops.gemm(h, self._w(p + ".net.2.weight"), bias=self._f(p + ".net.2.bias"), residual=tok)
 
     def _transformer(self, p, x, ctx, heads, F, dup=1):
@@ -449,17 +467,11 @@ class UNet3DConditionModel(ParamTreeModel):
         tok = ops.gemm(h.view(M, C), self._w1x1(p + ".proj_in.weight"), bias=self._f(p + ".proj_in.bias"))
         q = p + ".transformer_blocks.0"
         # self attention (attention.py:507)
-        # LayerNorm -> projection pairs (norm1 -> q/k/v, norm2 -> to_q, norm3 -> GEGLU): in tensor-core mode the norm is folded into
-        # the GEMM (one read-only statistics pass + epilogue terms, _ln_fold) instead of writing and re-reading a normalised copy
-        fold = ops.ln_fold_ok(tok.dtype, M, C)
+        # LayerNorm -> projection pairs (norm1 -> q/k/v, norm2 -> to_q, norm3 -> GEGLU): _ln_proj
         tc_attn = ops.self_attention_tc_ok(tok.dtype, HW, d)
         qkv_w = (lambda dtype=None: self._qkv_padded(q + ".attn1", heads, d, dtype=dtype)) if tc_attn else \
             (lambda dtype=None: self._cat_w(q + ".attn1", [q + ".attn1.to_q.weight", q + ".attn1.to_k.weight", q + ".attn1.to_v.weight"], dtype=dtype))
-        if fold:
-            w1_, cb1, _ = self._ln_fold(q + ".attn1.qkv" + (".pad" if tc_attn else ""), q + ".norm1", lambda: qkv_w(torch.float32))
-            qkv = ops.gemm(tok, w1_, bias=cb1, ln=ops.layernorm_stats(tok))
-        else:
-            qkv = ops.gemm(ops.layernorm(tok, self._f(q + ".norm1.weight"), self._f(q + ".norm1.bias")), qkv_w())
+        qkv = self._ln_proj(tok, q + ".norm1", q + ".attn1.qkv" + (".pad" if tc_attn else ""), lambda: qkv_w(torch.float32), lambda: (qkv_w(), None))
         if tc_attn:
             # tensor-core path: q/k heads zero-padded to 64 columns by the packed weight, V transposed per image (keys contiguous)
             qkv = qkv.view(NB, HW, 2 * heads * 64 + C)
@@ -476,12 +488,8 @@ class UNet3DConditionModel(ParamTreeModel):
             o = ops.attention(qkv[:, :, :C], qkv[:, :, C:2 * C], qkv[:, :, 2 * C:], heads, d ** -0.5)
         tok = ops.gemm(o.view(M, C), self._w(q + ".attn1.to_out.0.weight"), bias=self._f(q + ".attn1.to_out.0.bias"), residual=tok)
         # cross attention (attention.py:516-521; IPCrossAttention.forward :49-127); K/V of the context come from the per-clip cache
-        if fold:
-            w2_, cb2, _ = self._ln_fold(q + ".attn2.to_q", q + ".norm2", lambda: self._p(q + ".attn2.to_q.weight").detach())
-            qx = ops.gemm(tok, w2_, bias=cb2, ln=ops.layernorm_stats(tok)).view(NB, HW, C)
-        else:
-            n2 = ops.layernorm(tok, self._f(q + ".norm2.weight"), self._f(q + ".norm2.bias"))
-            qx = ops.gemm(n2, self._w(q + ".attn2.to_q.weight")).view(NB, HW, C)
+        qx = self._ln_proj(tok, q + ".norm2", q + ".attn2.to_q", lambda: self._p(q + ".attn2.to_q.weight").detach(),
+                           lambda: (self._w(q + ".attn2.to_q.weight"), None)).view(NB, HW, C)
         o = torch.empty((dup * NB, HW, C), dtype=qx.dtype, device=qx.device)
         L = ctx.ctx.shape[1]
         Bq = ctx.ctx.shape[0] // dup            # clips per context replica
@@ -510,23 +518,11 @@ class UNet3DConditionModel(ParamTreeModel):
                               k2=kvi[:, L - T:, :C], v2=kvi[:, L - T:, C:], alpha2=float(self._cfg["scale"]))
             else:
                 ops.attention(qx, kv_r[:, :, :C], kv_r[:, :, C:], heads, d ** -0.5, out=o_r, kv_batch_div=F)
-        w_o, b_o = self._w(q + ".attn2.to_out.0.weight"), self._f(q + ".attn2.to_out.0.bias")
-        if dup == 1:
-            tok = ops.gemm(o.view(M, C), w_o, bias=b_o, residual=tok)
-        else:                                   # the shared residual stream fans out here: same `tok` added to every replica's projection
-            tok_d = torch.empty((dup * M, C), dtype=tok.dtype, device=tok.device)
-            for r in range(dup):
-                ops.gemm(o[r * NB:(r + 1) * NB].view(M, C), w_o, bias=b_o, residual=tok, out=tok_d[r * M:(r + 1) * M])
-            tok = tok_d
+        # the shared residual stream fans out here: same `tok` added to every replica's projection
+        tok = self._gemm_replicas(o.view(dup * M, C), dup, self._w(q + ".attn2.to_out.0.weight"), bias=self._f(q + ".attn2.to_out.0.bias"), residual=tok)
         # feed forward (attention.py:563)
         tok = self._ff(q + ".ff", tok, q + ".norm3")
-        w_p, b_p = self._w1x1(p + ".proj_out.weight"), self._f(p + ".proj_out.bias")
-        if dup == 1:
-            out = ops.gemm(tok, w_p, bias=b_p, residual=res)
-        else:
-            out = torch.empty((dup * M, C), dtype=tok.dtype, device=tok.device)
-            for r in range(dup):
-                ops.gemm(tok[r * M:(r + 1) * M], w_p, bias=b_p, residual=res, out=out[r * M:(r + 1) * M])
+        out = self._gemm_replicas(tok, dup, self._w1x1(p + ".proj_out.weight"), bias=self._f(p + ".proj_out.bias"), residual=res)
         return out.view(dup * NB, H, W, C)
 
     def _motion(self, p, x, B, F):
@@ -549,18 +545,9 @@ class UNet3DConditionModel(ParamTreeModel):
                     pe = self._cached(("pe", a), lambda a=a: self._p(a + ".pos_encoder.pe").detach()[0].float().contiguous())
                 names = ["to_q", "to_k", "to_v"]
                 mk = lambda dtype=None, a=a: self._cat_w(a, [a + f".{nm}.weight" for nm in names], lora=[a + f".{nm}_lora" for nm in names], dtype=dtype)
-                if ops.ln_fold_ok(tok.dtype, M, C) and (pe is None or HW % 128 == 0):
-                    # (LN(x) + pe_f) Wqkv^T = LN-folded GEMM + the per-frame row-bias table pe Wqkv^T (motion_module.py:303,378)
-                    wq_, cb, rbt = self._ln_fold(a + ".qkv", q + f".norms.{j}", lambda: mk(torch.float32), pe=pe)
-                    rb = None
-                    if pe is not None:
-                        rb = self._cached(("pe_rb", a, B, F), lambda rbt=rbt: rbt[:F].repeat(B, 1).contiguous())      # row group = (clip, frame)
-                    qkv = ops.gemm(tok, wq_, bias=cb, rowbias=rb, rows_per_group=HW if pe is not None else 0,
-                                   ln=ops.layernorm_stats(tok)).view(B, F, HW, 3 * C)
-                else:
-                    n = ops.layernorm(tok, self._f(q + f".norms.{j}.weight"), self._f(q + f".norms.{j}.bias"), pe=pe,
-                                      rows_per_frame=HW, frames=F)
-                    qkv = ops.gemm(n, mk()).view(B, F, HW, 3 * C)
+                # (LN(x) + pe_f) Wqkv^T (motion_module.py:303,378)
+                qkv = self._ln_proj(tok, q + f".norms.{j}", a + ".qkv", lambda: mk(torch.float32), lambda: (mk(), None),
+                                    ok=pe is None or HW % 128 == 0, pe=pe, clips=B, frames=F, rows_per_frame=HW).view(B, F, HW, 3 * C)
                 o = ops.temporal_attention(qkv, heads, d ** -0.5)
                 wo = self._cat_w(a + ".out", [a + ".to_out.0.weight"], lora=[a + ".to_out_lora"])
                 tok = ops.gemm(o.view(M, C), wo, bias=self._f(a + ".to_out.0.bias"), residual=tok)
