@@ -1,5 +1,6 @@
 // Spatial self-attention and short-context cross-attention on Hopper tensor cores (wgmma), for the long-sequence, small-head
-// cases that dominate the UNet (level 0: 4096 tokens, 8 heads x 40 dims; level 1: 1024 tokens, head dim 80).
+// cases that dominate the UNet (SD-1.5: level 0 4096 tokens, 8 heads x 40 dims, level 1 1024 tokens, head dim 80; SD-2.x: head dim 64
+// at every level).
 //
 // Self-attention: one CTA = 128 query rows of one (image, head), two warpgroups of 64 rows each.  Per 128-key tile:
 //   S = Q K^T     wgmma m64n128k16, Q and K straight from 128B-swizzled TMA tiles, fp32 S in registers
@@ -7,7 +8,8 @@
 //   O += P V      wgmma m64nDVk16 with P (bf16) as the register A operand and V^T (keys contiguous) as the K-major B operand
 // K and V^T tiles arrive through a 2-stage TMA ring; the score matrix never leaves registers.
 // Operand prerequisites (prepared by the host side once per layer call, see unet.py::_transformer):
-//   q, k : [NB, L, heads * 64] bf16 (zero columns 40..63 per head come for free from zero rows in the packed projection weight)
+//   q, k : [NB, L, heads * 64] bf16 (zero columns 40..63 per head come for free from zero rows in the packed projection weight;
+//          head dim 64: the fused [q | k | v] projection as is, one 64-column atom per head, 4 k-steps)
 //          or, head dim 80, the fused [q | k | v] projection as is (two 64-column atoms per head, 5 k-steps)
 //   v^T  : [NB, heads * D, L] bf16 (fyc_transpose_tokens)
 //
@@ -102,7 +104,7 @@ struct AttnTcParams {
   float scale_log2e;
 };
 
-// KA: 64-column atoms per q / k head (1: D = 40 zero-padded to 64, 2: D = 80), KS: k-steps of QK^T that hold data, DV: PV accumulator
+// KA: 64-column atoms per q / k head (1: D = 40 zero-padded to 64 or D = 64, 2: D = 80), KS: k-steps of QK^T that hold data, DV: PV accumulator
 // columns (D rounded up to a multiple of 16 rows of V^T; the extra rows belong to the next head and only feed unstored columns)
 template <int KA, int KS, int DV, int D>
 __global__ void __launch_bounds__(NTHREADS, 1)
@@ -392,11 +394,11 @@ extern "C" int32_t fyc_transpose_tokens(const void* in, void* out, int64_t NB, i
   return FYC_OK;
 }
 
-// qk: [NB, L, ldqk] bf16 with q head h at columns [q_col0 + 64h, +64) and k head h at [k_col0 + 64h, +64) (cols D..63 zero);
-// vt: [NB, heads*D, L]; out: [NB, L, ldo] (head h at columns [h*D, (h+1)*D)).
+// qk: [NB, L, ldqk] bf16 with q head h at columns [q_col0 + 64h, +64) and k head h at [k_col0 + 64h, +64) (D = 40: cols 40..63 zero;
+// D = 64: the unpadded fused projection); vt: [NB, heads*D, L]; out: [NB, L, ldo] (head h at columns [h*D, (h+1)*D)).
 extern "C" int32_t fyc_self_attention_tc(const void* qk, int64_t ldqk, int64_t q_col0, int64_t k_col0, const void* vt, void* out,
                                          int64_t ldo, int64_t NB, int64_t heads, int64_t L, int64_t D, float scale, void* stream) {
-  FYC_CHECK(D == 40, "self_attention_tc: built for head dim 40 (got %lld)", (long long)D);
+  FYC_CHECK(D == 40 || D == 64, "self_attention_tc: built for head dims 40 and 64 (got %lld)", (long long)D);
   FYC_CHECK(L % 128 == 0 && L >= 128, "self_attention_tc: sequence length %lld must be a multiple of 128", (long long)L);
   FYC_CHECK(ldqk % 8 == 0 && q_col0 % 8 == 0 && k_col0 % 8 == 0 && ldo % 8 == 0, "self_attention_tc: 16-byte alignment");
   FYC_CHECK((((uintptr_t)qk | (uintptr_t)vt | (uintptr_t)out) & 15) == 0, "self_attention_tc: pointers must be 16-byte aligned");
@@ -414,13 +416,14 @@ extern "C" int32_t fyc_self_attention_tc(const void* qk, int64_t ldqk, int64_t q
   {
     uint64_t dims[3] = {(uint64_t)L, (uint64_t)(heads * D), (uint64_t)NB};
     uint64_t str[2] = {(uint64_t)L * 2, (uint64_t)L * heads * D * 2};
-    uint32_t box[3] = {64, 48, 1};
+    uint32_t box[3] = {64, D == 40 ? 48u : 64u, 1};
     int32_t rc = make_map(&mv, vt, 3, dims, str, box);
     if (rc) return rc;
   }
   AttnTcParams p;
   p.out = (bf16*)out; p.ldo = ldo; p.bso = L * ldo; p.L = (int)L; p.heads = (int)heads;
   p.scale_log2e = scale * 1.4426950408889634f;
+  if (D == 64) return launch_self<1, 4, 64, 64>(mq, mk, mv, p, NB, (cudaStream_t)stream);
   return launch_self<1, 3, 48, 40>(mq, mk, mv, p, NB, (cudaStream_t)stream);      // k-step 3 would multiply the zero columns 48..63
 }
 
@@ -460,24 +463,24 @@ extern "C" int32_t fyc_self_attention_tc_d80(const void* qkv, int64_t ldqkv, int
   return launch_self<2, 5, 80, 80>(mq, mk, mv, p, NB, (cudaStream_t)stream);
 }
 
-// Cross-attention with a resident short context on tensor cores (head dim 40 or 80).  q: [NB, Lq, ldq] bf16, head h at columns [q_col0 + D h, +D),
+// Cross-attention with a resident short context on tensor cores (head dim 40, 64 or 80).  q: [NB, Lq, ldq] bf16, head h at columns [q_col0 + D h, +D),
 // UNPADDED, ldq >= heads * D;
-// k: [NBc, 80, ldk] with head h at columns [DKP h, +D), DKP = 64 for D = 40 (columns D..63 ZERO) or 80 for D = 80, rows Lk..79 zero;
+// k: [NBc, 80, ldk] with head h at columns [DKP h, +D), DKP = 64 for D = 40 (columns D..63 ZERO) or 64, 80 for D = 80, rows Lk..79 zero;
 // vt: [NBc, heads * D, 80]; optional second context k2 [NBc, 16, ldk2], vt2 [NBc, heads * D, 16] (rows / columns Lk2..15 zero).
 // out[n, i, h D + :] = out_alpha softmax_j<Lk(scale q k^T) v + alpha2 softmax_j<Lk2(scale q k2^T) v2, NBc = NB / kv_batch_div.
 extern "C" int32_t fyc_cross_attention_tc(const void* q, int64_t ldq, int64_t q_col0, const void* k, int64_t ldk, const void* vt,
                                           const void* k2, int64_t ldk2, const void* vt2, void* out, int64_t ldo, int64_t NB, int64_t heads,
                                           int64_t Lq, int64_t D, int64_t Lk, int64_t Lk2, int64_t kv_batch_div, float scale, float out_alpha,
                                           float alpha2, void* stream) {
-  FYC_CHECK(D == 40 || D == 80, "cross_attention_tc: head dim %lld (40 or 80)", (long long)D);
+  FYC_CHECK(D == 40 || D == 64 || D == 80, "cross_attention_tc: head dim %lld (40, 64 or 80)", (long long)D);
   FYC_CHECK(Lk >= 1 && Lk <= CX_LK && Lk2 >= 0 && Lk2 <= CX_LK2 && Lq >= 1 && kv_batch_div >= 1 && NB % kv_batch_div == 0, "cross_attention_tc: bad shape");
   FYC_CHECK((k2 != nullptr) == (Lk2 > 0) && (vt2 != nullptr) == (Lk2 > 0), "cross_attention_tc: second context needs k2, vt2 and Lk2 > 0");
   FYC_CHECK(ldq % 8 == 0 && q_col0 % 8 == 0 && ldk % 8 == 0 && ldo % 8 == 0 && (k2 == nullptr || ldk2 % 8 == 0), "cross_attention_tc: 16-byte alignment");
   FYC_CHECK((((uintptr_t)q | (uintptr_t)k | (uintptr_t)vt | (uintptr_t)out | (uintptr_t)k2 | (uintptr_t)vt2) & 15) == 0, "cross_attention_tc: pointers must be 16-byte aligned");
   FYC_CHECK(NB < 65536 && heads < 65536, "cross_attention_tc: grid too large");
   const int64_t NBc = NB / kv_batch_div;
-  const int64_t DKP = D == 40 ? 64 : 80;
-  const uint32_t DV = D == 40 ? 48 : 80;
+  const int64_t DKP = D == 80 ? 80 : 64;
+  const uint32_t DV = D == 40 ? 48 : (uint32_t)D;
   CUtensorMap mq, mk, mv, mk2, mv2;
   {
     // q and k as 3-D maps over the WHOLE head-packed row (box origin = the head's first column): columns past the row end - the tail
@@ -527,6 +530,12 @@ extern "C" int32_t fyc_cross_attention_tc(const void* q, int64_t ldq, int64_t q_
   if (D == 40) {
     constexpr int smem = cx_smem<1, 48>();
     auto kern = attention_cx_kernel<1, 3, 48, 40>;
+    static bool attr = false;
+    if (!attr) { FYC_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem)); attr = true; }
+    kern<<<grid, NTHREADS, smem, st>>>(mq, mk, mv, mk2, mv2, p);
+  } else if (D == 64) {
+    constexpr int smem = cx_smem<1, 64>();
+    auto kern = attention_cx_kernel<1, 4, 64, 64>;
     static bool attr = false;
     if (!attr) { FYC_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem)); attr = true; }
     kern<<<grid, NTHREADS, smem, st>>>(mq, mk, mv, mk2, mv2, p);

@@ -361,11 +361,12 @@ def transpose_tokens(x, col0, C):
 
 
 def self_attention_tc_ok(dtype, L, D):
-    return _impl != L_SIMT and dtype == torch.bfloat16 and D == 40 and L % 128 == 0 and lib().fyc_tcgen05_available() == 1
+    return _impl != L_SIMT and dtype == torch.bfloat16 and D in (40, 64) and L % 128 == 0 and lib().fyc_tcgen05_available() == 1
 
 
 def self_attention_tc(qk, q_col0, k_col0, vt, heads, D, scale):
-    """tensor-core self-attention: qk [NB, L, ld] with 64-wide zero-padded q/k heads, vt [NB, heads*D, L] -> [NB, L, heads*D]."""
+    """tensor-core self-attention: qk [NB, L, ld] with 64-wide q/k heads (D = 40: zero-padded, D = 64: the fused projection as is),
+    vt [NB, heads*D, L] -> [NB, L, heads*D]."""
     NB, L, _ = qk.shape
     out = torch.empty((NB, L, heads * D), dtype=qk.dtype, device=qk.device)
     with _rec("attention_tc", 4.0 * NB * heads * L * L * D, qk.element_size() * (4 * NB * L * heads * D)):
@@ -398,12 +399,12 @@ CROSS_LK, CROSS_LK2 = 80, 16                                      # padded key c
 
 
 def cross_attention_tc_ok(dtype, D, Lk, Lk2):
-    return (use_cross_tc and _impl != L_SIMT and dtype == torch.bfloat16 and D in (40, 80) and 1 <= Lk <= CROSS_LK and 0 <= Lk2 <= CROSS_LK2
+    return (use_cross_tc and _impl != L_SIMT and dtype == torch.bfloat16 and D in (40, 64, 80) and 1 <= Lk <= CROSS_LK and 0 <= Lk2 <= CROSS_LK2
             and lib().fyc_tcgen05_available() == 1)
 
 
 def cross_dkp(D):
-    """column stride between the heads of the packed context keys: 64 (zero-padded heads) for D = 40, 80 for D = 80"""
+    """column stride between the heads of the packed context keys: 64 (zero-padded heads) for D = 40, D itself for D = 64 / 80"""
     return 64 if D == 40 else D
 
 

@@ -110,13 +110,19 @@ def unet_param_spec(cfg):
     def ff(p, c):
         lin(p + ".net.0.proj", 8 * c, c); lin(p + ".net.2", c, 4 * c)
 
+    def proj(p, c):             # Transformer3DModel proj_in / proj_out: Linear with use_linear_projection (SD-2.x), else a 1x1 conv
+        if cfg.get("use_linear_projection", False):
+            lin(p, c, c)
+        else:
+            conv(p, c, c, 1)
+
     def transformer(p, c):
-        norm(p + ".norm", c); conv(p + ".proj_in", c, c, 1)
+        norm(p + ".norm", c); proj(p + ".proj_in", c)
         q = p + ".transformer_blocks.0"
         attn(q + ".attn1", c, c); norm(q + ".norm1", c)
         attn(q + ".attn2", c, xd, cfg["use_ip_cross_attention"]); norm(q + ".norm2", c)
         ff(q + ".ff", c); norm(q + ".norm3", c)
-        conv(p + ".proj_out", c, c, 1)
+        proj(p + ".proj_out", c)
 
     def motion(p, c):
         p = p + ".temporal_transformer"
@@ -230,16 +236,24 @@ class UNet3DConditionModel(ParamTreeModel):
         super().__init__()
         kw = {k: v for k, v in locals().items() if k not in ("self", "unused", "__class__")}
         kw["motion_module_kwargs"] = dict(motion_module_kwargs or {})
+        # use_linear_projection (SD-2.x): proj_in / proj_out of every Transformer3DModel are Linear (C, C) instead of 1x1 convs
+        # (animatediff/models/attention.py:179-215,270-295) - the same GEMM on the channels-last tokens, only the key shapes differ.
+        # upcast_attention (SD-2.x) makes the reference form Q K^T and the softmax in fp32 (diffusers/models/attention.py:649-660).  Every
+        # engine attention kernel already does, whatever the storage dtype: the wgmma kernels (attention_tc.cu) and the mma.sync kernel
+        # (attention_mma.cu) accumulate S in fp32 registers and run the softmax on them, the SIMT kernel (attention_simt.cu) and the
+        # temporal kernels (temporal_mma.cu, attention_simt.cu) likewise; bf16 is only the operand and output format.  So the flag
+        # changes nothing here and is accepted as is.
         unsupported = dict(center_input_sample=False, only_cross_attention=False, dual_cross_attention=False,
-                           use_linear_projection=False, class_embed_type=None, num_class_embeds=None,
-                           upcast_attention=False, resnet_time_scale_shift="default", use_pseudo_conv3d=False,
+                           class_embed_type=None, num_class_embeds=None, resnet_time_scale_shift="default", use_pseudo_conv3d=False,
                            use_text_encoder_2=False, use_temporal_conv=False, downsample_padding=1,
                            mid_block_scale_factor=1, act_fn="silu")
         for k, v in unsupported.items():
             if kw[k] != v:
                 raise NotImplementedError(f"UNet3DConditionModel: {k}={kw[k]!r} is outside the shipped inference configs")
-        if unet_use_cross_frame_attention or unet_use_temporal_attention:
-            raise NotImplementedError("unet_use_cross_frame_attention / unet_use_temporal_attention are off in every shipped config")
+        if unet_use_cross_frame_attention:
+            raise NotImplementedError("UNet3DConditionModel: unet_use_cross_frame_attention is not built (off in every shipped config)")
+        if unet_use_temporal_attention:
+            raise NotImplementedError("UNet3DConditionModel: unet_use_temporal_attention (in-block temporal attention) is not built")
         if tuple(down_block_types) != ("CrossAttnDownBlock3D",) * (len(block_out_channels) - 1) + ("DownBlock3D",):
             raise NotImplementedError(f"down_block_types {down_block_types}")
         if use_motion_module and motion_module_type != "Vanilla":
@@ -249,8 +263,9 @@ class UNet3DConditionModel(ParamTreeModel):
                   temporal_attention_dim_div=1, zero_initialize=True, add_temporal_lora=False, rank=4,
                   use_rope_postion_encoding=False)
         mm.update(kw["motion_module_kwargs"])
-        if mm["temporal_attention_dim_div"] != 1 or mm["use_rope_postion_encoding"] or any(
-                t != "Temporal_Self" for t in mm["attention_block_types"]):
+        if mm["use_rope_postion_encoding"]:
+            raise NotImplementedError("UNet3DConditionModel: RoPE temporal position encoding (use_rope_postion_encoding) is not built")
+        if mm["temporal_attention_dim_div"] != 1 or any(t != "Temporal_Self" for t in mm["attention_block_types"]):
             raise NotImplementedError("motion module variant outside the shipped configs")
         self._mm = mm
         self.config = FrozenDict(dict(kw, _class_name="UNet3DConditionModel", _diffusers_version="0.11.1"))
@@ -274,8 +289,10 @@ class UNet3DConditionModel(ParamTreeModel):
 
     @classmethod
     def from_pretrained_2d(cls, pretrained_model_path, subfolder=None, unet_additional_kwargs=None):
-        """animatediff/models/unet.py:674-726: SD-1.5 2-D UNet folder (config.json + diffusion_pytorch_model.bin)
-        inflated to the 3-D model; conv_in zero-extended to 9 input channels when a concat condition is on."""
+        """animatediff/models/unet.py:674-726: SD-1.5 or SD-2.x 2-D UNet folder (config.json + diffusion_pytorch_model.bin)
+        inflated to the 3-D model; conv_in zero-extended to 9 input channels when a concat condition is on.  An SD-2.x config's
+        per-level ``attention_head_dim`` list, ``cross_attention_dim`` 1024, ``use_linear_projection`` and ``upcast_attention`` pass
+        through as they are."""
         unet_additional_kwargs = dict(unet_additional_kwargs or {})
         if subfolder is not None:
             pretrained_model_path = os.path.join(pretrained_model_path, subfolder)
@@ -469,13 +486,15 @@ class UNet3DConditionModel(ParamTreeModel):
         # self attention (attention.py:507)
         # LayerNorm -> projection pairs (norm1 -> q/k/v, norm2 -> to_q, norm3 -> GEGLU): _ln_proj
         tc_attn = ops.self_attention_tc_ok(tok.dtype, HW, d)
-        qkv_w = (lambda dtype=None: self._qkv_padded(q + ".attn1", heads, d, dtype=dtype)) if tc_attn else \
+        pad = tc_attn and d != 64          # head dim 64: every head already is one 64-column atom, the plain [q | k | v] stack is the layout
+        qkv_w = (lambda dtype=None: self._qkv_padded(q + ".attn1", heads, d, dtype=dtype)) if pad else \
             (lambda dtype=None: self._cat_w(q + ".attn1", [q + ".attn1.to_q.weight", q + ".attn1.to_k.weight", q + ".attn1.to_v.weight"], dtype=dtype))
-        qkv = self._ln_proj(tok, q + ".norm1", q + ".attn1.qkv" + (".pad" if tc_attn else ""), lambda: qkv_w(torch.float32), lambda: (qkv_w(), None))
+        qkv = self._ln_proj(tok, q + ".norm1", q + ".attn1.qkv" + (".pad" if pad else ""), lambda: qkv_w(torch.float32), lambda: (qkv_w(), None))
         if tc_attn:
-            # tensor-core path: q/k heads zero-padded to 64 columns by the packed weight, V transposed per image (keys contiguous)
+            # tensor-core path: q/k heads 64 columns apart (head dim 40: zero-padded by the packed weight), V transposed per image (keys contiguous)
             qkv = qkv.view(NB, HW, 2 * heads * 64 + C)
-            ops.note_padding(2.0 * M * C * 2 * heads * (64 - d))
+            if pad:
+                ops.note_padding(2.0 * M * C * 2 * heads * (64 - d))
             vt = ops.transpose_tokens(qkv, 2 * heads * 64, C)
             o = ops.self_attention_tc(qkv, 0, heads * 64, vt, heads, d, d ** -0.5)
         elif ops.self_attention_tc80_ok(tok.dtype, HW, d):
@@ -494,7 +513,7 @@ class UNet3DConditionModel(ParamTreeModel):
         L = ctx.ctx.shape[1]
         Bq = ctx.ctx.shape[0] // dup            # clips per context replica
         ipx = self._cfg["use_ip_cross_attention"]
-        for r in range(dup if p in ctx.kx else 0):       # tensor-core path (head dims 40 / 80): resident packed context, text + image keys in one launch
+        for r in range(dup if p in ctx.kx else 0):       # tensor-core path (head dims 40 / 64 / 80): resident packed context, text + image keys in one launch
             T = self._cfg["num_tokens"] if ipx else 0
             sc = d ** -0.5 if (self._xformers_semantics or not ipx) else float(self._cfg["scale"])     # reference quirk, see below
             kvp, vt = (t[r * Bq:(r + 1) * Bq] for t in ctx.kx[p])
@@ -592,7 +611,7 @@ class UNet3DConditionModel(ParamTreeModel):
         kv, kvi, kx, kxi = {}, {}, {}, {}
         ip = self._cfg["use_ip_cross_attention"]
         T = self._cfg["num_tokens"] if ip else 0
-        # tensor-core cross-attention (head dims 40 / 80): the text tokens zero-padded to 80 keys, the image tokens to 16, projected with the
+        # tensor-core cross-attention (head dims 40 / 64 / 80): the text tokens zero-padded to 80 keys, the image tokens to 16, projected with the
         # per-head padded K weight, V transposed so that the keys are contiguous - once per clip, read by every step
         pad_t = pad_i = None
         for p in self._transformer_prefixes():
@@ -794,7 +813,7 @@ class UNet2DConditionOutput:
 
 
 class UNet2DConditionModel(UNet3DConditionModel):
-    """Stock SD-1.5 ``UNet2DConditionModel`` (diffusers/models/unet_2d_condition.py:44-439) on the engine - the T2I first-frame
+    """Stock SD-1.5 / SD-2.x ``UNet2DConditionModel`` (diffusers/models/unet_2d_condition.py:44-439) on the engine - the T2I first-frame
     generator of scripts/inference.py:195-204,300-306 (`pipeline_base`, SURVEY 8f row 3).  It is the 3-D model without motion
     modules run on one frame: an inflated conv on F = 1 is the 2-D conv, cross-frame GroupNorm over one frame is the per-image
     GroupNorm, and the state-dict keys are the 2-D checkpoint's own (``from_pretrained_2d`` relies on exactly that).  Same
@@ -831,7 +850,7 @@ class UNet2DConditionModel(UNet3DConditionModel):
 
     @classmethod
     def from_pretrained(cls, pretrained_model_path, subfolder=None, **kwargs):
-        """config.json + diffusion_pytorch_model.bin of an SD-1.5 ``unet/`` folder (diffusers/modeling_utils.py:from_pretrained)."""
+        """config.json + diffusion_pytorch_model.bin of an SD-1.5 or SD-2.x ``unet/`` folder (diffusers/modeling_utils.py:from_pretrained)."""
         if subfolder is not None:
             pretrained_model_path = os.path.join(pretrained_model_path, subfolder)
         with open(os.path.join(pretrained_model_path, "config.json")) as f:

@@ -174,11 +174,11 @@ int32_t fyc_attention(const fyc_attention_args* a, void* stream);
  * '(b f) d c -> (b d) f c' regrouping (motion_module.py:376,462) is absorbed into the addressing. */
 int32_t fyc_temporal_attention(const void* qkv, void* out, int64_t B, int64_t F, int64_t HW, int64_t heads,
                                int64_t D, float scale, int32_t dtype, void* stream);
-/* Spatial self-attention on the tensor cores (wgmma; S, O accumulators in registers) for head dim 40, L % 128 == 0 - the level-0
- * attn1 of the UNet (diffusers/models/attention.py:649-678 via animatediff/models/attention.py:507).  qk: [NB, L, ldqk]
- * bf16, q head h at columns [q_col0 + 64h, +64), k head h at [k_col0 + 64h, +64), columns D..63 of each head ZERO (zero
- * rows in the packed projection weight); vt: [NB, heads*D, L] (V transposed per image, fyc_transpose_tokens);
- * out: [NB, L, ldo], head h at columns [h*D, (h+1)*D). */
+/* Spatial self-attention on the tensor cores (wgmma; S, O accumulators in registers) for head dim 40 or 64, L % 128 == 0 - the level-0
+ * attn1 of an SD-1.5 UNet, every attn1 of an SD-2.x UNet (diffusers/models/attention.py:649-678 via animatediff/models/attention.py:507).
+ * qk: [NB, L, ldqk] bf16, q head h at columns [q_col0 + 64h, +64), k head h at [k_col0 + 64h, +64): for D = 40 columns 40..63 of each
+ * head ZERO (zero rows in the packed projection weight), for D = 64 the fused [q | k | v] projection as is; vt: [NB, heads*D, L]
+ * (V transposed per image, fyc_transpose_tokens); out: [NB, L, ldo], head h at columns [h*D, (h+1)*D). */
 int32_t fyc_self_attention_tc(const void* qk, int64_t ldqk, int64_t q_col0, int64_t k_col0, const void* vt, void* out,
                               int64_t ldo, int64_t NB, int64_t heads, int64_t L, int64_t D, float scale, void* stream);
 /* The same for head dim 80, L % 256 == 0 - the level-1 attn1 (1024 tokens at cfg2, 2304 at cfg5).  qkv: [NB, L, ldqkv] bf16, the fused
@@ -187,7 +187,7 @@ int32_t fyc_self_attention_tc(const void* qk, int64_t ldqk, int64_t q_col0, int6
  * columns past the last k head (the v block does).  vt: [NB, heads * 80, L]; out: [NB, L, ldo]. */
 int32_t fyc_self_attention_tc_d80(const void* qkv, int64_t ldqkv, int64_t q_col0, int64_t k_col0, const void* vt, void* out,
                                   int64_t ldo, int64_t NB, int64_t heads, int64_t L, float scale, void* stream);
-/* Cross-attention against a SHORT, step-invariant context on the tensor cores (head dim 40 or 80; bf16): attn2 of every transformer block
+/* Cross-attention against a SHORT, step-invariant context on the tensor cores (head dim 40, 64 or 80; bf16): attn2 of every transformer block
  * (diffusers/models/attention.py:649-678) and, with the second context, the whole IP-Adapter cross-attention in one launch
  * (animatediff/models/attention.py:92-120, ip_adapter/attention_processor.py:137-168):
  *   out[n, i, h D + :] = out_alpha softmax_{j < Lk}(scale q k^T) v + alpha2 softmax_{j < Lk2}(scale q k2^T) v2,   context n / kv_batch_div.
@@ -195,7 +195,8 @@ int32_t fyc_self_attention_tc_d80(const void* qkv, int64_t ldqkv, int64_t q_col0
  * O live in registers, the probabilities are normalised in registers (one key tile: no online rescaling) and both contexts accumulate into ONE
  * O accumulator, written once.  Operands, packed once per clip by the caller:
  *   q   [NB, Lq, ldq], head h at columns [q_col0 + D h, +D), unpadded;
- *   k   [NBc, 80, ldk], head h at columns [DKP h, +D) with DKP = 64 for D = 40 (columns D..63 of every head ZERO) | 80 for D = 80, rows Lk..79 zero;
+ *   k   [NBc, 80, ldk], head h at columns [DKP h, +D) with DKP = 64 for D = 40 (columns D..63 of every head ZERO) | 64 for D = 64 | 80 for
+ *       D = 80, rows Lk..79 zero;
  *   vt  [NBc, heads D, 80] (V transposed: keys contiguous), columns Lk..79 zero;
  *   k2  [NBc, 16, ldk2], vt2 [NBc, heads D, 16] likewise (NULL / Lk2 = 0: no second context). */
 int32_t fyc_cross_attention_tc(const void* q, int64_t ldq, int64_t q_col0, const void* k, int64_t ldk, const void* vt, const void* k2,
