@@ -4,11 +4,14 @@
 //
 // One persistent CTA per SM, 9 warps:
 //   warp 8 (1 lane)  TMA producer : cp.async.bulk.tensor (4-D box for the activation patch, 3-D box for the weight slab) into a
-//                                   4-stage 128B-swizzled shared-memory ring, mbarrier expect_tx
+//                                   3- or 4-stage 128B-swizzled shared-memory ring, mbarrier expect_tx
 //   warps 0..7       two consumer warpgroups, 64 rows of the 128-row tile each: wgmma.mma_async m64 x BN x 16 (bf16 -> fp32
 //                    register accumulators) straight from the swizzled stages, then the fused epilogue (bias / time-embedding
-//                    row bias / residual / GEGLU / LayerNorm fold / alpha) on the registers and direct global stores.
+//                    row bias / residual / GEGLU / LayerNorm fold / alpha) on the registers into the warpgroup's own shared-memory
+//                    staging buffer, which one thread writes out with TMA stores (clipped at the output's true extent).
 // The producer runs ahead across tile boundaries, so the next tile's operands stream in while the consumers run the epilogue.
+// The residual half-tile is TMA-loaded into the staging buffer at the start of the tile, so it lands during the mainloop; the
+// TMA stores of a tile drain while the warpgroup runs the next tile's MMAs.
 // The 3x3 convolution never builds an im2col matrix: for each filter tap the producer loads the SAME 4-D box shifted
 // by (dy, dx); TMA's out-of-bounds zero fill implements the padding halo.  A plain GEMM is the 1-tap special case.
 // Stride-2 convolutions run on a parity-plane split of the input (fyc_space_to_planes), which turns every tap into
@@ -22,14 +25,17 @@ namespace {
 
 constexpr int BM = 128;            // rows (output pixels) per tile: two warpgroups x 64
 constexpr int BK = 64;             // K per stage = one 128-byte swizzle row of bf16
-constexpr int STAGES = 4;
-constexpr int MAX_BN = 256;
+constexpr int STAGES = 4;          // plain-mode stages when the ring has room for them
 constexpr int A_BYTES = BM * BK * 2;           // 16 KB
-constexpr int B_BYTES = MAX_BN * BK * 2;       // 32 KB
-constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
 constexpr int MAX_STAGES = 8;                   // barrier slots; the W-resident mode runs up to 8 A-only stages
-constexpr int RING_BYTES = STAGES * STAGE_BYTES;                // 192 KB operand ring (or W slab + A ring)
-constexpr int SMEM_BYTES = RING_BYTES + 256 + 1024;              // + barriers + slack to align the ring to 1024 B
+constexpr int MAX_RING_BYTES = 192 * 1024;      // operand ring (or W slab + A ring): 4 stages of a BN = 256 tile
+constexpr int SMEM_LIMIT = 232448;              // 227 KB: the per-block opt-in maximum of sm_90
+constexpr int SMEM_EXTRA = 256 + 1024;          // barriers + slack to align the ring to 1024 B
+// Output staging: each warpgroup writes its 64-row half-tile into its own buffer as 32-byte-wide column boxes (16 bf16 or 8 fp32
+// columns, 64 rows x 32 B = 2 KB each, CU_TENSOR_MAP_SWIZZLE_32B).  Every BN is a multiple of 16, so a tile is a whole number of
+// boxes and no box reaches into the next tile's columns; a warp's 4- or 8-byte fragment stores hit 32 distinct banks per wavefront.
+constexpr int OUT_BOX_BYTES = 32;
+constexpr int OUT_BOX_SMEM = 64 * OUT_BOX_BYTES;   // 2 KB
 constexpr int NUM_THREADS = 288;          // 2 consumer warpgroups + the TMA warp
 
 struct TcParams {
@@ -43,9 +49,9 @@ struct TcParams {
   int lg_bw, lg_bh;          // log2 of bw, bh (both powers of two)
   int64_t m_tiles;
   int tap_dy[9], tap_dx[9], tap_img[9];
-  // epilogue
-  const float* bias; const void* residual; const float* rowbias; void* out;
-  int64_t ldo, ldr, rows_per_group;
+  // epilogue; the output and residual are addressed by their tensor maps
+  const float* bias; const float* rowbias;
+  int64_t rows_per_group;
   int64_t ldrb;              // row stride of rowbias (elements; N unless the caller passes a slice of a wider table)
   float alpha;
   int flags;
@@ -55,6 +61,11 @@ struct TcParams {
   const float* ln_rs;
   // W-resident mode (small K): the CTA keeps its whole BN x K weight slab in shared memory and only streams A
   int resident, a_stages;
+  // shared memory: [operand ring: ring_bytes][staging warpgroup 0 | 1: stg_bytes each][barriers]
+  int ring_bytes, stg_bytes;
+  // output / residual box origin of warpgroup 1's half-tile relative to warpgroup 0's, in (w, h, image): the patch is halved
+  // along its outermost dimension that is wider than 1
+  int half_dw, half_dh, half_dn;
 };
 
 // ---------------------------------------------------------------------------------------------- PTX wrappers
@@ -92,6 +103,22 @@ __device__ __forceinline__ void tma_load_3d(const CUtensorMap* map, uint64_t* ba
       ::"r"(smem_u32(dst)), "l"(reinterpret_cast<uint64_t>(map)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2)
       : "memory");
 }
+__device__ __forceinline__ void tma_store_4d(const CUtensorMap* map, const void* src, int c0, int c1, int c2, int c3) {
+  asm volatile("cp.async.bulk.tensor.4d.global.shared::cta.bulk_group [%0, {%2, %3, %4, %5}], [%1];"
+               ::"l"(reinterpret_cast<uint64_t>(map)), "r"(smem_u32(src)), "r"(c0), "r"(c1), "r"(c2), "r"(c3) : "memory");
+}
+__device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
+// the committed stores have finished reading shared memory (their source may be overwritten)
+__device__ __forceinline__ void bulk_wait_read() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
+// the committed stores are complete
+__device__ __forceinline__ void bulk_wait_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
+// generic-proxy writes to shared memory become visible to the TMA (async proxy) reads that follow
+__device__ __forceinline__ void fence_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
+// named barrier over one consumer warpgroup (id 0 is __syncthreads)
+__device__ __forceinline__ void warpgroup_sync(int wg) {
+  if (wg == 0) asm volatile("bar.sync 1, 128;" ::: "memory");
+  else asm volatile("bar.sync 2, 128;" ::: "memory");
+}
 
 // ---------------------------------------------------------------------------------------------- tile coordinates
 struct TileCoord { int n, w, h, i; };   // n block; patch column / row / image-group of the 128-pixel m block
@@ -116,26 +143,34 @@ __device__ __forceinline__ int64_t tile_pixel(const TcParams& p, const TileCoord
 }
 
 // ---------------------------------------------------------------------------------------------- epilogue
+// Byte offset of (row, col) of a half-tile in the staging layout: column box col / (32 / esize), then row, in the 32-byte
+// swizzle TMA applies (16-byte chunk index XOR row bit 2; the staging buffers are 1024-byte aligned).
+__device__ __forceinline__ uint32_t stage_off(int row, int col, int esize) {
+  const int cpb = OUT_BOX_BYTES / esize;
+  const uint32_t in_box = (uint32_t)(row * OUT_BOX_BYTES + (col % cpb) * esize);
+  return (uint32_t)(col / cpb) * OUT_BOX_SMEM + (in_box ^ (((in_box >> 7) & 1u) << 4));
+}
+
 // The accumulator of warpgroup wg holds rows wg*64 + 16*warp + lane/4 (+8) of the tile; n-tile j (8 columns) sits in acc[4j .. 4j+3]:
-// columns 8j + 2(lane%4) + {0, 1} of the first row, then of the second.
+// columns 8j + 2(lane%4) + {0, 1} of the first row, then of the second.  The results go to the warpgroup's staging buffer `stg`,
+// which holds the residual half-tile on entry when there is one; each thread reads its residual where it then writes its result.
 template <int BN>
-__device__ __forceinline__ void epilogue(const TcParams& p, const TileCoord& c, const float* acc, int wg, int warp4, int lane) {
+__device__ __forceinline__ void epilogue(const TcParams& p, const TileCoord& c, const float* acc, int wg, int warp4, int lane, uint8_t* stg) {
   const int q = lane & 3;
-  const int rbase = wg * 64 + warp4 * 16 + (lane >> 2);
   const int flags = p.flags;
   const bool geglu = flags & FYC_EPI_GEGLU, out_f32 = flags & FYC_EPI_OUT_F32, lnf = flags & FYC_EPI_LNFOLD;
   const bool has_bias = flags & FYC_EPI_BIAS, has_res = flags & FYC_EPI_RESIDUAL, has_rb = flags & FYC_EPI_ROWBIAS;
 #pragma unroll
   for (int half = 0; half < 2; ++half) {
-    const int64_t pix = tile_pixel(p, c, rbase + 8 * half);
-    if (pix < 0) continue;
+    const int row = warp4 * 16 + (lane >> 2) + 8 * half;       // row of the warpgroup's 64-row half-tile
+    const int64_t pix = tile_pixel(p, c, wg * 64 + row);
+    if (pix < 0) continue;                                      // beyond M: the TMA store clips the row
     const float rs = lnf ? __ldg(p.ln_rs + pix) : 1.0f;
     const float* rb = has_rb ? p.rowbias + (pix / p.rows_per_group) * p.ldrb : nullptr;
     if (geglu) {
       if constexpr (BN == 256) {
         // columns [0,128) of the tile are `a`, [128,256) the matching gate (weight rows pre-interleaved per 128 outputs)
         const float* bp = p.bias + c.n * 256;
-        bf16* o = reinterpret_cast<bf16*>(p.out) + pix * p.ldo + c.n * 128;
 #pragma unroll
         for (int j = 0; j < 16; ++j) {
           const int col = 8 * j + 2 * q;
@@ -145,7 +180,7 @@ __device__ __forceinline__ void epilogue(const TcParams& p, const TileCoord& c, 
           const float g0 = acc[4 * (j + 16) + 2 * half], g1 = acc[4 * (j + 16) + 2 * half + 1];
           const float x = fmaf(a0, rs, ba.x) * gelu_erf_fast(fmaf(g0, rs, bg.x));
           const float y = fmaf(a1, rs, ba.y) * gelu_erf_fast(fmaf(g1, rs, bg.y));
-          *reinterpret_cast<__nv_bfloat162*>(o + col) = __floats2bfloat162_rn(x, y);
+          *reinterpret_cast<__nv_bfloat162*>(stg + stage_off(row, col, 2)) = __floats2bfloat162_rn(x, y);
         }
       }
       continue;
@@ -153,20 +188,19 @@ __device__ __forceinline__ void epilogue(const TcParams& p, const TileCoord& c, 
     const float scale = lnf ? rs : p.alpha;
 #pragma unroll
     for (int j = 0; j < BN / 8; ++j) {
-      const int n = c.n * BN + 8 * j + 2 * q;
+      const int col = 8 * j + 2 * q, n = c.n * BN + col;
       if (n >= p.N) continue;
       float x = acc[4 * j + 2 * half] * scale, y = acc[4 * j + 2 * half + 1] * scale;
       if (has_bias) { const float2 b = __ldg(reinterpret_cast<const float2*>(p.bias + n)); x += b.x; y += b.y; }
       if (has_rb) { const float2 b = __ldg(reinterpret_cast<const float2*>(rb + n)); x += b.x; y += b.y; }
       if (out_f32) {
-        if (has_res) { const float2 r = *reinterpret_cast<const float2*>(reinterpret_cast<const float*>(p.residual) + pix * p.ldr + n); x += r.x; y += r.y; }
-        *reinterpret_cast<float2*>(reinterpret_cast<float*>(p.out) + pix * p.ldo + n) = make_float2(x, y);
+        float2* s = reinterpret_cast<float2*>(stg + stage_off(row, col, 4));
+        if (has_res) { const float2 r = *s; x += r.x; y += r.y; }
+        *s = make_float2(x, y);
       } else {
-        if (has_res) {
-          const float2 r = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(reinterpret_cast<const bf16*>(p.residual) + pix * p.ldr + n));
-          x += r.x; y += r.y;
-        }
-        *reinterpret_cast<__nv_bfloat162*>(reinterpret_cast<bf16*>(p.out) + pix * p.ldo + n) = __floats2bfloat162_rn(x, y);
+        __nv_bfloat162* s = reinterpret_cast<__nv_bfloat162*>(stg + stage_off(row, col, 2));
+        if (has_res) { const float2 r = __bfloat1622float2(*s); x += r.x; y += r.y; }
+        *s = __floats2bfloat162_rn(x, y);
       }
     }
   }
@@ -176,20 +210,21 @@ __device__ __forceinline__ void epilogue(const TcParams& p, const TileCoord& c, 
 template <int BN>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
 gemm_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_w, const __grid_constant__ CUtensorMap map_a2,
-               const TcParams p) {
+               const __grid_constant__ CUtensorMap map_out, const __grid_constant__ CUtensorMap map_res, const TcParams p) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);     // SWIZZLE_128B operands need 1024-byte alignment
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + RING_BYTES);
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + p.ring_bytes + 2 * p.stg_bytes);
   uint64_t* full = bars;                       // [MAX_STAGES]
   uint64_t* empty = bars + MAX_STAGES;         // [MAX_STAGES]
   uint64_t* wbar = bars + 2 * MAX_STAGES;      // W-resident mode: the weight slab has landed
+  uint64_t* rbar = wbar + 1;                   // [2] the residual half-tile of warpgroup 0 / 1 has landed in its staging buffer
   // operand ring, two layouts:
-  //   plain     [A 16 KB | W BN x 128 B (<= 32 KB)] x 4 stages
+  //   plain     [A 16 KB | W BN x 128 B] x a_stages
   //   resident  [W slab k_iters x BN x 128 B][A 16 KB x a_stages]
-  const int nstages = p.resident ? p.a_stages : STAGES;
+  const int nstages = p.a_stages;
   const uint32_t slab_kb = (uint32_t)BN * (BK * 2);
   const uint32_t a_base = p.resident ? (uint32_t)(p.taps * p.cin_blocks) * slab_kb : 0u;
-  const uint32_t a_stride = p.resident ? (uint32_t)A_BYTES : (uint32_t)STAGE_BYTES;
+  const uint32_t a_stride = p.resident ? (uint32_t)A_BYTES : (uint32_t)A_BYTES + slab_kb;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int k_iters = p.taps * p.cin_blocks;
   const int64_t num_tiles = p.m_tiles * p.n_tiles;
@@ -197,6 +232,7 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
   if (threadIdx.x == 0) {
     for (int s = 0; s < MAX_STAGES; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 256); }   // empty: one arrival per consumer thread
     mbar_init(wbar, 1);
+    mbar_init(&rbar[0], 1); mbar_init(&rbar[1], 1);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
   __syncthreads();
@@ -237,10 +273,39 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
   }
   // ==================================================================== consumer warpgroups
   const int wg = warp >> 2, warp4 = warp & 3;
+  // Everything below except rphase is re-derived from the kernel parameters where it is used, so that it does not hold registers
+  // across the mainloop (BN = 256 needs 128 of the 168 for its accumulator).
+  const bool elected = (threadIdx.x & 127) == 0;                // issues the warpgroup's TMA stores / residual loads
+  auto stg = [&]() { return smem + p.ring_bytes + wg * p.stg_bytes; };
+  const bool has_res = p.flags & FYC_EPI_RESIDUAL;
+  auto cpb = [&]() { return (p.flags & FYC_EPI_OUT_F32) ? OUT_BOX_BYTES / 4 : OUT_BOX_BYTES / 2; };
+  if (elected) {
+    asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&map_out)) : "memory");
+    if (has_res) asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&map_res)) : "memory");
+  }
   float acc[BN / 2];
-  int stage = 0; uint32_t phase = 0;
+  int stage = 0; uint32_t phase = 0, rphase = 0;
   if (p.resident) mbar_wait(wbar, 0);
+  // this warpgroup's half of tile t: output columns [col0, col0 + nbox * cpb), box origin (bw0, bh0, bn0); live is false only for
+  // the rows past M of a plain GEMM's last tile.  Evaluated before and again after the mainloop, so nothing of it stays in registers
+  // across the MMAs.
+  auto half_tile = [&](int64_t t, int& col0, int& nbox, int& bw0, int& bh0, int& bn0) {
+    const TileCoord tc = tile_coord(p, t);
+    const int bn_out = (p.flags & FYC_EPI_GEGLU) ? BN / 2 : BN;
+    col0 = tc.n * bn_out;
+    nbox = min(bn_out, p.N_out - col0) / cpb();
+    bw0 = tc.w * p.bw + wg * p.half_dw; bh0 = tc.h * p.bh + wg * p.half_dh; bn0 = tc.i * p.bn + wg * p.half_dn;
+    return tile_pixel(p, tc, wg * 64) >= 0;
+  };
   for (int64_t tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+    if (has_res && elected) {
+      int col0, nbox, bw0, bh0, bn0;
+      if (half_tile(tile, col0, nbox, bw0, bh0, bn0)) {
+        bulk_wait_read();                                        // the previous tile's stores have read the staging buffer
+        mbar_expect_tx(&rbar[wg], (uint32_t)(nbox * OUT_BOX_SMEM));
+        for (int b = 0; b < nbox; ++b) tma_load_4d(&map_res, &rbar[wg], stg() + b * OUT_BOX_SMEM, col0 + b * cpb(), bw0, bh0, bn0);
+      }
+    }
     int prev = -1;
     for (int k = 0; k < k_iters; ++k) {
       mbar_wait(&full[stage], phase);
@@ -260,8 +325,21 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
     wgmma_wait<0>();
     wgmma_fence_regs<BN / 2>(acc);
     mbar_arrive(&empty[prev]);
-    epilogue<BN>(p, tile_coord(p, tile), acc, wg, warp4, lane);
+    int col0, nbox, bw0, bh0, bn0;
+    if (!half_tile(tile, col0, nbox, bw0, bh0, bn0)) continue;
+    if (elected) bulk_wait_read();
+    warpgroup_sync(wg);                                          // the staging buffer is free (and holds the residual, if any)
+    if (has_res) { mbar_wait(&rbar[wg], rphase); rphase ^= 1; }
+    epilogue<BN>(p, tile_coord(p, tile), acc, wg, warp4, lane, stg());
+    fence_async_smem();
+    warpgroup_sync(wg);
+    if (elected) {
+      for (int b = 0; b < nbox; ++b) tma_store_4d(&map_out, stg() + b * OUT_BOX_SMEM, col0 + b * cpb(), bw0, bh0, bn0);
+      bulk_commit();
+    }
   }
+  // no CTA may exit while its TMA stores still read its shared memory
+  if (elected) bulk_wait_all();
 }
 
 // parity-plane split for stride-2 convolutions: x [NB, H, W, C] -> planes [4, NB, H/2, W/2, C], plane = 2*(h&1) + (w&1)
@@ -300,14 +378,15 @@ EncodeTiledFn get_encode_fn() {
 }
 
 int32_t encode_map(CUtensorMap* m, const void* base, int rank, const uint64_t* dims, const uint64_t* strides_bytes,
-                   const uint32_t* box) {
+                   const uint32_t* box, CUtensorMapDataType dtype = CU_TENSOR_MAP_DATA_TYPE_BFLOAT16,
+                   CUtensorMapSwizzle swizzle = CU_TENSOR_MAP_SWIZZLE_128B) {
   EncodeTiledFn fn = get_encode_fn();
   FYC_CHECK(fn != nullptr, "tensor-core path: cuTensorMapEncodeTiled driver entry point unavailable");
   cuuint64_t gdim[5]; cuuint64_t gstr[4]; cuuint32_t bx[5]; cuuint32_t es[5];
   for (int i = 0; i < rank; ++i) { gdim[i] = dims[i]; bx[i] = box[i]; es[i] = 1; }
   for (int i = 0; i + 1 < rank; ++i) gstr[i] = strides_bytes[i];
-  CUresult r = fn(m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, (cuuint32_t)rank, const_cast<void*>(base), gdim, gstr, bx, es,
-                  CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
+  CUresult r = fn(m, dtype, (cuuint32_t)rank, const_cast<void*>(base), gdim, gstr, bx, es,
+                  CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
                   CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   FYC_CHECK(r == CUDA_SUCCESS, "cuTensorMapEncodeTiled failed with CUresult %d (rank %d dims %llu %llu %llu %llu)", (int)r, rank,
             (unsigned long long)dims[0], (unsigned long long)dims[1], (unsigned long long)(rank > 2 ? dims[2] : 0),
@@ -315,50 +394,86 @@ int32_t encode_map(CUtensorMap* m, const void* base, int rank, const uint64_t* d
   return FYC_OK;
 }
 
+// Output (or residual) map of a launch: `cols` channels by W x H x NB pixels at `base`, pixel (w, h, n) at element offset
+// w * sw + h * sh + n * sn.  The dimensions are the tensor's true extent, so TMA clips the rows past M and the columns past N_out.
+// Box: one 32-byte column box of a warpgroup's half patch (choose_tiles sets the split).
+int32_t encode_out_map(CUtensorMap* m, const void* base, const TcParams& p, uint64_t cols, uint64_t W, uint64_t H, uint64_t NB,
+                       uint64_t sw, uint64_t sh, uint64_t sn) {
+  const bool f32 = (p.flags & FYC_EPI_OUT_F32) != 0;
+  const uint64_t es = f32 ? 4 : 2;
+  uint64_t dims[4] = {cols, W, H, NB};
+  uint64_t str[3] = {sw * es, sh * es, sn * es};
+  uint32_t box[4] = {(uint32_t)(OUT_BOX_BYTES / es), (uint32_t)(p.half_dw ? p.half_dw : p.bw), (uint32_t)(p.half_dh ? p.half_dh : p.bh),
+                     (uint32_t)(p.half_dn ? p.half_dn : p.bn)};
+  return encode_map(m, base, 4, dims, str, box, f32 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16,
+                    CU_TENSOR_MAP_SWIZZLE_32B);
+}
+
 // accumulator widths with a kernel instantiation (wgmma N)
 constexpr int BN_CHOICES[] = {256, 192, 160, 128, 96, 80, 64, 48, 32, 16};
+// fp32 output: BN <= 128 keeps a warpgroup's staging buffer (64 x BN x 4 B) within 32 KB
+constexpr int MAX_BN_F32 = 128;
 
-int pick_bn(int64_t N, bool geglu) {
+int pick_bn(int64_t N, bool geglu, bool f32) {
   if (geglu) return 256;
   for (int bn : BN_CHOICES)
-    if (N % bn == 0) return bn;
+    if (N % bn == 0 && (!f32 || bn <= MAX_BN_F32)) return bn;
   return 16;                            // N % 16 == 0 checked by the caller
+}
+
+// Shared-memory budget of one CTA (227 KB opt-in = 232 448 B):
+//   staging  2 x 64 x BN_out x (2 or 4 B)  <= 64 KB  (bf16 BN = 256: 2 x 32 KB; GEGLU: 2 x 16 KB; fp32 BN <= 128: 2 x 32 KB)
+//   barriers + alignment slack  1 280 B
+//   operand ring  the rest rounded down to 1 KB, at most 192 KB: bf16 BN = 256 -> 161 KB (3 plain stages of 48 KB),
+//                 BN = 160 -> 185 KB (4 plain stages of 36 KB; W-resident K = 320: 100 KB slab + 5 A stages), GEGLU -> 192 KB
+int stg_bytes_for(int bn, int flags) {
+  const int bn_out = (flags & FYC_EPI_GEGLU) ? bn / 2 : bn;
+  return 64 * bn_out * ((flags & FYC_EPI_OUT_F32) ? 4 : 2);
+}
+int ring_bytes_for(int bn, int flags) {
+  const int avail = (SMEM_LIMIT - SMEM_EXTRA - 2 * stg_bytes_for(bn, flags)) & ~1023;
+  return avail < MAX_RING_BYTES ? avail : MAX_RING_BYTES;
 }
 
 // Tile width, operand-staging mode and grid for one launch.
 //  * default: the largest instantiated BN <= 256 dividing N (fewest re-reads of the A tiles through L2);
 //  * few rounds of tiles per SM (small M): BN that minimises rounds x (BN + fixed cost) - a 2.2-round launch at BN = 256 runs as
-//    3 full rounds, the same problem at a narrower BN as more, shorter rounds (ragged last N tile is zero-filled by TMA and guarded
-//    in the epilogue);
-//  * small K (k_iters x BN x 128 B <= 128 KB) and many tiles per CTA: W-resident - the grid is rounded down to a multiple of
-//    n_tiles so a CTA's n block is fixed, its weight slab is loaded once, and the ring streams only A (L2 -> SM traffic per tile
-//    drops from (128 + BN) x K to 128 x K elements).
+//    3 full rounds, the same problem at a narrower BN as more, shorter rounds (ragged last N tile is zero-filled by TMA and clipped
+//    by the output map);
+//  * small K (the slab k_iters x BN x 128 B leaves room for >= 3 A stages) and many tiles per CTA: W-resident - the grid is
+//    rounded down to a multiple of n_tiles so a CTA's n block is fixed, its weight slab is loaded once, and the ring streams only A
+//    (L2 -> SM traffic per tile drops from (128 + BN) x K to 128 x K elements).
+// Also sets the shared-memory split and the warpgroup half of the output patch.
 void choose_tiles(TcParams& p, int* grid_out) {
   const int sms = fyc_sm_count();
-  const bool geglu = (p.flags & FYC_EPI_GEGLU) != 0;
+  const bool geglu = (p.flags & FYC_EPI_GEGLU) != 0, f32 = (p.flags & FYC_EPI_OUT_F32) != 0;
+  const int max_bn = f32 ? MAX_BN_F32 : 256;
   const int k_iters = p.taps * p.cin_blocks;
-  p.resident = 0; p.a_stages = STAGES;
-  p.BN = pick_bn(p.N, geglu);
+  p.resident = 0;
+  p.BN = pick_bn(p.N, geglu, f32);
   p.n_tiles = (int)ceil_div64(p.N, p.BN);
+  p.half_dw = p.half_dh = p.half_dn = 0;
+  if (p.bn >= 2) p.half_dn = p.bn / 2;
+  else if (p.bh >= 2) p.half_dh = p.bh / 2;
+  else p.half_dw = p.bw / 2;
+  int grid = 0;
   if (!geglu) {
     // W-resident candidate
     int rbn = 0;
-    for (int min_stages = 4; min_stages >= 3 && !rbn; --min_stages)      // prefer a slab that leaves the full 4-stage A ring; settle for 3
+    for (int min_stages = 4; min_stages >= 3 && !rbn; --min_stages)      // prefer a slab that leaves a 4-stage A ring; settle for 3
       for (int bn : BN_CHOICES)
-        if (bn >= 128 && p.N % bn == 0 && (int64_t)k_iters * bn * 128 <= RING_BYTES - min_stages * A_BYTES) { rbn = bn; break; }
+        if (bn >= 128 && bn <= max_bn && p.N % bn == 0 &&
+            (int64_t)k_iters * bn * 128 <= ring_bytes_for(bn, p.flags) - min_stages * A_BYTES) { rbn = bn; break; }
     if (rbn) {
       const int nt = p.N / rbn;
-      const int grid = (sms / nt) * nt;
-      if (nt <= sms && grid * 16 >= sms * 15 && p.m_tiles * nt >= (int64_t)grid * 4) {
+      const int rgrid = (sms / nt) * nt;
+      if (nt <= sms && rgrid * 16 >= sms * 15 && p.m_tiles * nt >= (int64_t)rgrid * 4) {
         p.resident = 1; p.BN = rbn; p.n_tiles = nt;
-        int st = (int)((RING_BYTES - (int64_t)k_iters * rbn * 128) / A_BYTES);
-        p.a_stages = st > MAX_STAGES ? MAX_STAGES : st;
-        *grid_out = grid;
-        return;
+        grid = rgrid;
       }
     }
     const int64_t rounds0 = ceil_div64(p.m_tiles * p.n_tiles, sms);
-    if (rounds0 < 8) {
+    if (!p.resident && rounds0 < 8) {
       // per k block a tile costs max(MMA, operand feed) clocks: 128 x bn x 64 MACs at 1024 MAC/clk per SM (H100 dense bf16), and
       // (128 + bn) x 128 B of operands at ~24 B/clk per SM of L2 bandwidth, plus a fixed per-tile overhead (epilogue, pipeline fill)
       auto cost_of = [&](int bn, int64_t nt) {
@@ -367,32 +482,47 @@ void choose_tiles(TcParams& p, int* grid_out) {
       };
       int64_t best = cost_of(p.BN, p.n_tiles);
       for (int bn : BN_CHOICES) {
-        if (bn > p.N || bn < 64) continue;
+        if (bn > p.N || bn < 64 || bn > max_bn) continue;
         const int64_t nt = ceil_div64(p.N, bn);
         const int64_t cost = cost_of(bn, nt);
         if (cost < best) { best = cost; p.BN = bn; p.n_tiles = (int)nt; }
       }
     }
   }
-  const int64_t tiles = p.m_tiles * p.n_tiles;
-  *grid_out = (int)(tiles < sms ? tiles : sms);
+  p.stg_bytes = stg_bytes_for(p.BN, p.flags);
+  p.ring_bytes = ring_bytes_for(p.BN, p.flags);
+  const int slab = k_iters * p.BN * 128;
+  const int st = p.resident ? (p.ring_bytes - slab) / A_BYTES : p.ring_bytes / (A_BYTES + p.BN * 128);
+  p.a_stages = st > (p.resident ? MAX_STAGES : STAGES) ? (p.resident ? MAX_STAGES : STAGES) : st;
+  if (!p.resident) {
+    const int64_t tiles = p.m_tiles * p.n_tiles;
+    grid = (int)(tiles < sms ? tiles : sms);
+  }
+  *grid_out = grid;
 }
 
 template <int BN>
-int32_t launch_bn(const CUtensorMap& ma, const CUtensorMap& mw, const CUtensorMap& ma2, const TcParams& p, int grid, cudaStream_t st) {
+int32_t launch_bn(const CUtensorMap& ma, const CUtensorMap& mw, const CUtensorMap& ma2, const CUtensorMap& mo, const CUtensorMap& mr,
+                  const TcParams& p, int grid, cudaStream_t st) {
   static bool attr_set = false;
   if (!attr_set) {
-    FYC_CUDA(cudaFuncSetAttribute(gemm_tc_kernel<BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES));
+    FYC_CUDA(cudaFuncSetAttribute(gemm_tc_kernel<BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_LIMIT));
     attr_set = true;
   }
-  gemm_tc_kernel<BN><<<grid, NUM_THREADS, SMEM_BYTES, st>>>(ma, mw, ma2, p);
+  const int smem = p.ring_bytes + 2 * p.stg_bytes + SMEM_EXTRA;
+  FYC_CHECK(smem <= SMEM_LIMIT && p.a_stages >= 2 && p.a_stages <= MAX_STAGES, "tensor-core GEMM: shared-memory plan does not fit (BN %d)", BN);
+  gemm_tc_kernel<BN><<<grid, NUM_THREADS, smem, st>>>(ma, mw, ma2, mo, mr, p);
   FYC_LAUNCH_CHECK();
   return FYC_OK;
 }
 
-int32_t launch_tc(const CUtensorMap& ma, const CUtensorMap& mw, TcParams p, int grid, cudaStream_t st, const CUtensorMap* ma2p = nullptr) {
+// mr: the residual map (FYC_EPI_RESIDUAL only; otherwise unused)
+int32_t launch_tc(const CUtensorMap& ma, const CUtensorMap& mw, const CUtensorMap& mo, const CUtensorMap* mr, TcParams p, int grid,
+                  cudaStream_t st, const CUtensorMap* ma2p = nullptr) {
   const CUtensorMap& ma2 = ma2p ? *ma2p : ma;
+  const CUtensorMap& mres = mr ? *mr : mo;
   if (!ma2p) p.cb_split = 0x7fffffff;
+  FYC_CHECK(!(p.flags & FYC_EPI_RESIDUAL) || mr, "tensor-core GEMM: residual epilogue without a residual map");
   FYC_CHECK((p.bw & (p.bw - 1)) == 0 && (p.bh & (p.bh - 1)) == 0 && p.bw > 0 && p.bh > 0, "tensor-core GEMM: patch dims must be powers of two");
   p.lg_bw = 0; while ((1 << p.lg_bw) < p.bw) ++p.lg_bw;
   p.lg_bh = 0; while ((1 << p.lg_bh) < p.bh) ++p.lg_bh;
@@ -400,16 +530,16 @@ int32_t launch_tc(const CUtensorMap& ma, const CUtensorMap& mw, TcParams p, int 
   FYC_CHECK(tiles < (1ll << 31) && p.M < (1ll << 31) && p.rows_per_group < (1ll << 31), "tensor-core GEMM: problem exceeds the 32-bit tile index range");
   if (grid > tiles) grid = (int)tiles;
   switch (p.BN) {
-    case 256: return launch_bn<256>(ma, mw, ma2, p, grid, st);
-    case 192: return launch_bn<192>(ma, mw, ma2, p, grid, st);
-    case 160: return launch_bn<160>(ma, mw, ma2, p, grid, st);
-    case 128: return launch_bn<128>(ma, mw, ma2, p, grid, st);
-    case 96: return launch_bn<96>(ma, mw, ma2, p, grid, st);
-    case 80: return launch_bn<80>(ma, mw, ma2, p, grid, st);
-    case 64: return launch_bn<64>(ma, mw, ma2, p, grid, st);
-    case 48: return launch_bn<48>(ma, mw, ma2, p, grid, st);
-    case 32: return launch_bn<32>(ma, mw, ma2, p, grid, st);
-    case 16: return launch_bn<16>(ma, mw, ma2, p, grid, st);
+    case 256: return launch_bn<256>(ma, mw, ma2, mo, mres, p, grid, st);
+    case 192: return launch_bn<192>(ma, mw, ma2, mo, mres, p, grid, st);
+    case 160: return launch_bn<160>(ma, mw, ma2, mo, mres, p, grid, st);
+    case 128: return launch_bn<128>(ma, mw, ma2, mo, mres, p, grid, st);
+    case 96: return launch_bn<96>(ma, mw, ma2, mo, mres, p, grid, st);
+    case 80: return launch_bn<80>(ma, mw, ma2, mo, mres, p, grid, st);
+    case 64: return launch_bn<64>(ma, mw, ma2, mo, mres, p, grid, st);
+    case 48: return launch_bn<48>(ma, mw, ma2, mo, mres, p, grid, st);
+    case 32: return launch_bn<32>(ma, mw, ma2, mo, mres, p, grid, st);
+    case 16: return launch_bn<16>(ma, mw, ma2, mo, mres, p, grid, st);
   }
   FYC_CHECK(false, "tensor-core GEMM: no kernel for BN = %d", p.BN);
 }
@@ -484,12 +614,20 @@ int32_t fyc_gemm_tc(const fyc_gemm_args* g, cudaStream_t st) {
     }
     FYC_CHECK(g->M < (1ll << 31), "gemm(tensor cores): M too large");
     p.bias = g->bias; p.rowbias = g->rowbias; p.rows_per_group = g->rows_per_group > 0 ? g->rows_per_group : 1; p.ldrb = g->N;
-    p.residual = g->residual ? (f32 ? (const void*)((const float*)g->residual + b * g->strideO) : (const void*)((const bf16*)g->residual + b * g->strideO)) : nullptr;
-    p.out = f32 ? (void*)((float*)g->out + b * g->strideO) : (void*)((bf16*)g->out + b * g->strideO);
-    p.ldo = g->ldo; p.ldr = g->ldr; p.alpha = g->alpha; p.flags = g->epilogue;
+    p.alpha = g->alpha;
     p.ln_rs = g->ln_rowstats;
     p.cb_split = g->A2 ? (int)(g->K1 / BK) : 0x7fffffff;
-    int32_t rc = launch_tc(ma, mw, p, grid, st, g->A2 ? &ma2 : nullptr);
+    // output / residual: N_out x M rows of ldo / ldr elements (ldo may exceed N_out: the caller passes a column slice)
+    const int64_t es = f32 ? 4 : 2;
+    const uint64_t M = (uint64_t)g->M, No = (uint64_t)p.N_out;
+    CUtensorMap mo, mr;
+    int32_t rc = encode_out_map(&mo, (const char*)g->out + b * g->strideO * es, p, No, M, 1, 1, g->ldo, g->ldo * M, g->ldo * M);
+    if (rc) return rc;
+    if (g->epilogue & FYC_EPI_RESIDUAL) {
+      rc = encode_out_map(&mr, (const char*)g->residual + b * g->strideO * es, p, No, M, 1, 1, g->ldr, g->ldr * M, g->ldr * M);
+      if (rc) return rc;
+    }
+    rc = launch_tc(ma, mw, mo, (g->epilogue & FYC_EPI_RESIDUAL) ? &mr : nullptr, p, grid, st, g->A2 ? &ma2 : nullptr);
     if (rc) return rc;
   }
   return FYC_OK;
@@ -524,7 +662,6 @@ int32_t fyc_conv3x3_tc(const fyc_conv3x3_args* c, const void* x_planes, cudaStre
   FYC_CHECK(fyc_conv3x3_tc_eligible(c), "conv3x3(tensor cores): shape/alignment not eligible");
   const int s = c->stride;
   const int64_t Ho = c->H / s, Wo = c->W / s;
-  const bool f32 = (c->epilogue & FYC_EPI_OUT_F32) != 0;
   TcParams p{};
   pick_patch(c->NB, Ho, Wo, &p.bw, &p.bh, &p.bn);
   p.M = c->NB * Ho * Wo; p.N = (int)c->Cout; p.N_out = p.N;
@@ -565,20 +702,27 @@ int32_t fyc_conv3x3_tc(const fyc_conv3x3_args* c, const void* x_planes, cudaStre
     int32_t rc = encode_map(&mw, c->w, 3, dims, str, box);
     if (rc) return rc;
   }
-  p.bias = c->bias; p.rowbias = c->rowbias; p.residual = c->residual; p.out = c->out;
+  p.bias = c->bias; p.rowbias = c->rowbias;
   p.ldrb = c->ld_rowbias > 0 ? c->ld_rowbias : c->Cout;
   p.rows_per_group = (c->images_per_group > 0 ? c->images_per_group : 1) * Ho * Wo;
-  p.ldo = c->Cout; p.ldr = c->Cout; p.alpha = 1.0f; p.flags = c->epilogue;
-  (void)f32;
-  return launch_tc(ma, mw, p, grid, st);
+  p.alpha = 1.0f;
+  const uint64_t C = (uint64_t)c->Cout;
+  CUtensorMap mo, mr;
+  int32_t rc = encode_out_map(&mo, c->out, p, C, Wo, Ho, c->NB, C, C * Wo, C * Wo * Ho);
+  if (rc) return rc;
+  if (c->epilogue & FYC_EPI_RESIDUAL) {
+    rc = encode_out_map(&mr, c->residual, p, C, Wo, Ho, c->NB, C, C * Wo, C * Wo * Ho);
+    if (rc) return rc;
+  }
+  return launch_tc(ma, mw, mo, (c->epilogue & FYC_EPI_RESIDUAL) ? &mr : nullptr, p, grid, st);
 }
 
 // nearest-x2 upsample + padded 3x3 conv as four 2x2-tap implicit GEMMs on the low-resolution image (fyc.h: w_phases).
 // Phase (py, px) produces output pixels (2*oh + py, 2*ow + px).  No kernel change is needed: the A boxes are the usual shifted
 // patches of x (TMA zero fill = the conv's zero padding, because an upsampled halo pixel is out of bounds exactly when its source
-// pixel is), and the interleaved destination is expressed through the epilogue's own address arithmetic - it computes
-// pix = (img * Ho + oh) * Wo + ow and stores at out + pix * ldo: with Wo := 2 W, ldo := 2 Cout and out advanced by
-// (py * 2W + px) * Cout that is ((img * 2H + 2 oh + py) * 2W + 2 ow + px) * Cout, the NHWC offset of the upsampled pixel.
+// pixel is), and the interleaved destination is a strided output map: base out + (py * 2W + px) * Cout, dimensions
+// {Cout, W, H, NB} with strides 2 Cout, 4W Cout, 4HW Cout elements, so low-resolution pixel (ow, oh, img) lands at
+// ((img * 2H + 2 oh + py) * 2W + 2 ow + px) * Cout, the NHWC offset of the upsampled pixel.
 bool fyc_conv3x3_up2_tc_eligible(const fyc_conv3x3_args* c) {
   if (c->dtype != FYC_BF16 || c->upsample != 2 || c->stride != 1 || c->pad_mode != 0 || !c->w_phases) return false;
   if (c->Cin % 8 || c->Cout % 16) return false;
@@ -600,10 +744,9 @@ int32_t fyc_conv3x3_up2_tc(const fyc_conv3x3_args* c, cudaStream_t st) {
   p.m_tiles = (int64_t)p.w_tiles * p.h_tiles * (c->NB / p.bn);
   p.flags = c->epilogue;
   int grid = 0;
-  choose_tiles(p, &grid);                       // tile shape / staging mode from the true (low-resolution) problem size
-  p.Wo = (int)(2 * W); p.M = c->NB * H * 2 * W;  // epilogue addressing only (see above); every ow < W < Wo, every pix < M
-  p.ldo = 2 * c->Cout; p.ldr = p.ldo; p.alpha = 1.0f;
-  p.bias = c->bias; p.rowbias = nullptr; p.residual = nullptr; p.rows_per_group = 1; p.ldrb = p.N;
+  choose_tiles(p, &grid);
+  p.alpha = 1.0f;
+  p.bias = c->bias; p.rowbias = nullptr; p.rows_per_group = 1; p.ldrb = p.N;
   CUtensorMap ma;
   {
     uint64_t dims[4] = {(uint64_t)c->Cin, (uint64_t)W, (uint64_t)H, (uint64_t)c->NB};
@@ -624,8 +767,11 @@ int32_t fyc_conv3x3_up2_tc(const fyc_conv3x3_args* c, cudaStream_t st) {
     uint32_t box[3] = {BK, 1, (uint32_t)p.BN};
     int32_t rc = encode_map(&mw, wp, 3, dims, str, box);
     if (rc) return rc;
-    p.out = (bf16*)c->out + ((int64_t)py * 2 * W + px) * c->Cout;
-    rc = launch_tc(ma, mw, p, grid, st);
+    const uint64_t C = (uint64_t)c->Cout;
+    CUtensorMap mo;
+    rc = encode_out_map(&mo, (const bf16*)c->out + ((int64_t)py * 2 * W + px) * c->Cout, p, C, W, H, c->NB, 2 * C, 4 * W * C, 4 * H * W * C);
+    if (rc) return rc;
+    rc = launch_tc(ma, mw, mo, nullptr, p, grid, st);
     if (rc) return rc;
   }
   return FYC_OK;
