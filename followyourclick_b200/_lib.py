@@ -11,7 +11,7 @@ import torch
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libfyc_sm90a.so")
 
-F32, BF16 = 0, 1
+F32, BF16, F16 = 0, 1, 2
 IMPL_AUTO, IMPL_SIMT, IMPL_TC = 0, 1, 2
 EPI_BIAS, EPI_RESIDUAL, EPI_ROWBIAS, EPI_GEGLU, EPI_OUT_F32, EPI_LNFOLD = 1, 2, 4, 8, 16, 32
 PRED = {"epsilon": 0, "sample": 1, "v_prediction": 2}
@@ -63,9 +63,13 @@ SIGNATURES = {
     "fyc_attention": (_i32, [C.POINTER(AttnArgs), _vp]),
     "fyc_temporal_attention": (_i32, [_vp, _vp, _i64, _i64, _i64, _i64, _i64, _f32, _i32, _vp]),
     "fyc_self_attention_tc": (_i32, [_vp, _i64, _i64, _i64, _vp, _vp, _i64, _i64, _i64, _i64, _i64, _f32, _vp]),
+    "fyc_self_attention_tc_f16": (_i32, [_vp, _i64, _i64, _i64, _vp, _vp, _i64, _i64, _i64, _i64, _i64, _f32, _vp]),
     "fyc_self_attention_tc_d80": (_i32, [_vp, _i64, _i64, _i64, _vp, _vp, _i64, _i64, _i64, _i64, _f32, _vp]),
+    "fyc_self_attention_tc_d80_f16": (_i32, [_vp, _i64, _i64, _i64, _vp, _vp, _i64, _i64, _i64, _i64, _f32, _vp]),
     "fyc_cross_attention_tc": (_i32, [_vp, _i64, _i64, _vp, _i64, _vp, _vp, _i64, _vp, _vp, _i64, _i64, _i64, _i64, _i64, _i64, _i64, _i64, _f32, _f32,
                                       _f32, _vp]),
+    "fyc_cross_attention_tc_f16": (_i32, [_vp, _i64, _i64, _vp, _i64, _vp, _vp, _i64, _vp, _vp, _i64, _i64, _i64, _i64, _i64, _i64, _i64, _i64, _f32,
+                                          _f32, _f32, _vp]),
     "fyc_transpose_tokens": (_i32, [_vp, _vp, _i64, _i64, _i64, _i64, _i64, _vp]),
     "fyc_softmax_rows": (_i32, [_vp, _vp, _i64, _i64, _i32, _vp]),
     "fyc_timestep_embed": (_i32, [_vp, _vp, _vp, _i64, _i64, _i32, _vp]),
@@ -122,6 +126,8 @@ def dtype_code(t):
         return F32
     if t == torch.bfloat16:
         return BF16
+    if t == torch.float16:
+        return F16
     raise FycError(f"unsupported activation dtype {t}")
 
 

@@ -1,7 +1,7 @@
-// Fused multi-head attention on tensor cores (bf16 operands, fp32 accumulation, online softmax in registers):
+// Fused multi-head attention on tensor cores (bf16 or fp16 operands, fp32 accumulation, online softmax in registers):
 // spatial self-attention (N up to 9216 keys), text cross-attention (77 keys) and the IP-adapter pass (4/16 keys).
 // The score matrix lives only in registers: S = Q K^T (mma.sync m16n8k16) -> warp-shuffle row max/sum ->
-// P (bf16, re-used in place as the A operand) -> O += P V.  K/V tiles are double-buffered with cp.async.
+// P (16-bit, re-used in place as the A operand) -> O += P V.  K/V tiles are double-buffered with cp.async.
 // Head dims 40/80/160 (SD-1.5: C/8) are padded to 48/80/160 in shared memory only.
 //
 // It serves the shapes the wgmma kernels of attention_tc.cu do not take (head dim 160, ragged or unpacked contexts).
@@ -28,58 +28,49 @@ __device__ __forceinline__ void ldmatrix_x4_trans(uint32_t* r, const void* p) {
   unsigned a = (unsigned)__cvta_generic_to_shared(p);
   asm volatile("ldmatrix.sync.aligned.m8n8.x4.trans.shared.b16 {%0, %1, %2, %3}, [%4];" : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]) : "r"(a));
 }
-__device__ __forceinline__ void mma_bf16(float* c, const uint32_t* a, uint32_t b0, uint32_t b1) {
-  asm volatile("mma.sync.aligned.m16n8k16.row.col.f32.bf16.bf16.f32 {%0, %1, %2, %3}, {%4, %5, %6, %7}, {%8, %9}, {%0, %1, %2, %3};"
-               : "+f"(c[0]), "+f"(c[1]), "+f"(c[2]), "+f"(c[3])
-               : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
-}
 // single MUFU.EX2 (exp2f() adds denormal-range handling: ~4 instructions per element in an issue-bound kernel)
 __device__ __forceinline__ float ex2_approx(float x) {
   float y;
   asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
   return y;
 }
-__device__ __forceinline__ uint32_t pack_bf16(float lo, float hi) {
-  __nv_bfloat162 v = __floats2bfloat162_rn(lo, hi);
-  return *reinterpret_cast<uint32_t*>(&v);
-}
 
 // copy a [64 x DP] tile (rows row0.., valid while < L, columns < D; everything else zero) into smem
-template <int D, int DP, int LDS, bool ONES_COL = false>
-__device__ __forceinline__ void load_tile(bf16* dst, const bf16* src, int64_t ld, int64_t row0, int64_t L, int tid) {
+template <int D, int DP, int LDS, bool ONES_COL = false, typename T>
+__device__ __forceinline__ void load_tile(T* dst, const T* src, int64_t ld, int64_t row0, int64_t L, int tid) {
   constexpr int CH = DP / 8;
   for (int i = tid; i < 64 * CH; i += NTHR) {
     int r = i / CH, c = (i % CH) * 8;
     bool ok = (row0 + r < L) && (c < D);
     if (ONES_COL && c == D) {
       // V padding chunk: [1, 0, 0, ...] for valid keys (row sum via the PV MMA), zeros for keys past the end
-      uint4 v = make_uint4((row0 + r < L) ? 0x00003F80u : 0u, 0u, 0u, 0u);     // bf16(1.0) = 0x3F80 in the low half
+      uint4 v = make_uint4((row0 + r < L) ? Pair16<T>::ONE : 0u, 0u, 0u, 0u);     // T(1.0) in the low half
       *reinterpret_cast<uint4*>(dst + r * LDS + c) = v;
       continue;
     }
-    const bf16* s = ok ? src + (row0 + r) * ld + c : src;
+    const T* s = ok ? src + (row0 + r) * ld + c : src;
     cp_async16(dst + r * LDS + c, s, ok ? 16 : 0);
   }
 }
 
-template <int D, int DP>
+template <int D, int DP, typename T>
 __global__ void __launch_bounds__(NTHR) attention_mma_kernel(fyc_attention_args a) {
   constexpr int LDS = DP + 8;          // padded row stride: ldmatrix row addresses hit distinct bank groups
   constexpr int KS = DP / 16;          // k-steps of QK^T
   constexpr int NO = DP / 8;           // n-tiles of the output
   constexpr bool ONES = DP > D;        // V's first padding column (col D) holds ones -> O[:, D] accumulates the softmax row sum
   extern __shared__ __align__(16) unsigned char smem_raw[];
-  bf16* sQ = reinterpret_cast<bf16*>(smem_raw);
-  bf16* sK = sQ + 64 * LDS;            // [2][64][LDS]
-  bf16* sV = sK + 2 * 64 * LDS;        // [2][64][LDS]
+  T* sQ = reinterpret_cast<T*>(smem_raw);
+  T* sK = sQ + 64 * LDS;            // [2][64][LDS]
+  T* sV = sK + 2 * 64 * LDS;        // [2][64][LDS]
   const int tid = threadIdx.x, lane = tid & 31, w = tid >> 5;
   const int g = lane >> 2, t = lane & 3;
   const int64_t n = blockIdx.z, h = blockIdx.y;
   const int64_t q0 = (int64_t)blockIdx.x * BQ;
   const int64_t nk = n / a.kv_batch_div;
-  const bf16* qg = (const bf16*)a.q + n * a.bsq + h * D;
-  const bf16* kg = (const bf16*)a.k + nk * a.bsk + h * D;
-  const bf16* vg = (const bf16*)a.v + nk * a.bsv + h * D;
+  const T* qg = (const T*)a.q + n * a.bsq + h * D;
+  const T* kg = (const T*)a.k + nk * a.bsk + h * D;
+  const T* vg = (const T*)a.v + nk * a.bsv + h * D;
   const int nkt = (int)((a.Lk + BKV - 1) / BKV);
 
   load_tile<D, DP, LDS>(sQ, qg, a.ldq, q0, a.Lq, tid);
@@ -110,8 +101,8 @@ __global__ void __launch_bounds__(NTHR) attention_mma_kernel(fyc_attention_args 
       for (int ks = 0; ks < KS; ++ks)
         ldmatrix_x4(qf[ks], sQ + (w * 16 + (lane & 15)) * LDS + ks * 16 + (lane >> 4) * 8);
     }
-    const bf16* kb = sK + buf * 64 * LDS;
-    const bf16* vb = sV + buf * 64 * LDS;
+    const T* kb = sK + buf * 64 * LDS;
+    const T* vb = sV + buf * 64 * LDS;
     // ---- S = Q K^T : 16 x 64 per warp
     float s[8][4];
 #pragma unroll
@@ -123,8 +114,8 @@ __global__ void __launch_bounds__(NTHR) attention_mma_kernel(fyc_attention_args 
         uint32_t b[4];
         const int mi = lane >> 3;
         ldmatrix_x4(b, kb + (jp * 16 + (lane & 7) + (mi >> 1) * 8) * LDS + ks * 16 + (mi & 1) * 8);
-        mma_bf16(s[2 * jp], qf[ks], b[0], b[1]);
-        mma_bf16(s[2 * jp + 1], qf[ks], b[2], b[3]);
+        mma16816<T>(s[2 * jp], qf[ks], b[0], b[1]);
+        mma16816<T>(s[2 * jp + 1], qf[ks], b[2], b[3]);
       }
     }
     // ---- online softmax on the raw scores (rows g, g+8; this thread holds cols 8j + 2t, +1).
@@ -158,8 +149,8 @@ __global__ void __launch_bounds__(NTHR) attention_mma_kernel(fyc_attention_args 
       float p0 = ex2_approx(fmaf(s[j][0], sl2, nb0)), p1 = ex2_approx(fmaf(s[j][1], sl2, nb0));
       float p2 = ex2_approx(fmaf(s[j][2], sl2, nb1)), p3 = ex2_approx(fmaf(s[j][3], sl2, nb1));
       if constexpr (!ONES) { rs0 += p0 + p1; rs1 += p2 + p3; }
-      pf[j >> 1][(j & 1) * 2 + 0] = pack_bf16(p0, p1);
-      pf[j >> 1][(j & 1) * 2 + 1] = pack_bf16(p2, p3);
+      pf[j >> 1][(j & 1) * 2 + 0] = pack_u32<T>(p0, p1);
+      pf[j >> 1][(j & 1) * 2 + 1] = pack_u32<T>(p2, p3);
     }
     if constexpr (!ONES) {
       rs0 += __shfl_xor_sync(0xffffffffu, rs0, 1); rs0 += __shfl_xor_sync(0xffffffffu, rs0, 2);
@@ -176,8 +167,8 @@ __global__ void __launch_bounds__(NTHR) attention_mma_kernel(fyc_attention_args 
         uint32_t b[4];
         const int mi = lane >> 3;
         ldmatrix_x4_trans(b, vb + (kk * 16 + (lane & 7) + (mi & 1) * 8) * LDS + np * 16 + (mi >> 1) * 8);
-        mma_bf16(o[2 * np], pf[kk], b[0], b[1]);
-        mma_bf16(o[2 * np + 1], pf[kk], b[2], b[3]);
+        mma16816<T>(o[2 * np], pf[kk], b[0], b[1]);
+        mma16816<T>(o[2 * np + 1], pf[kk], b[2], b[3]);
       }
     }
     __syncthreads();
@@ -189,23 +180,23 @@ __global__ void __launch_bounds__(NTHR) attention_mma_kernel(fyc_attention_args 
     l1 = __shfl_sync(0xffffffffu, o[NTL][2], (lane & ~3) | SRC);
   }
   const float i0 = a.out_alpha / l0, i1 = a.out_alpha / l1;
-  bf16* og = (bf16*)a.out + n * a.bso + h * D;
+  T* og = (T*)a.out + n * a.bso + h * D;
   const int64_t r0 = q0 + w * 16 + g, r1 = r0 + 8;
 #pragma unroll
   for (int i = 0; i < NO; ++i) {
     const int col = i * 8 + 2 * t;
     if (col < D) {
       if (r0 < a.Lq) {
-        __nv_bfloat162* dst = reinterpret_cast<__nv_bfloat162*>(og + r0 * a.ldo + col);
+        typename Pair16<T>::type* dst = reinterpret_cast<typename Pair16<T>::type*>(og + r0 * a.ldo + col);
         float x = o[i][0] * i0, y = o[i][1] * i0;
-        if (a.accumulate) { float2 e = __bfloat1622float2(*dst); x += e.x; y += e.y; }
-        *dst = __floats2bfloat162_rn(x, y);
+        if (a.accumulate) { float2 e = Pair16<T>::unpack(*dst); x += e.x; y += e.y; }
+        *dst = Pair16<T>::pack(x, y);
       }
       if (r1 < a.Lq) {
-        __nv_bfloat162* dst = reinterpret_cast<__nv_bfloat162*>(og + r1 * a.ldo + col);
+        typename Pair16<T>::type* dst = reinterpret_cast<typename Pair16<T>::type*>(og + r1 * a.ldo + col);
         float x = o[i][2] * i1, y = o[i][3] * i1;
-        if (a.accumulate) { float2 e = __bfloat1622float2(*dst); x += e.x; y += e.y; }
-        *dst = __floats2bfloat162_rn(x, y);
+        if (a.accumulate) { float2 e = Pair16<T>::unpack(*dst); x += e.x; y += e.y; }
+        *dst = Pair16<T>::pack(x, y);
       }
     }
   }
@@ -224,25 +215,25 @@ __global__ void __launch_bounds__(NTHR) attention_mma_kernel(fyc_attention_args 
 // the image keys and the kernel writes  out_alpha * softmax(q K_t^T s) V_t + alpha2 * softmax(q K_i^T s) V_i  ONCE - the reference's
 // two attention passes + add, without the second launch, the second read of Q, or a read-modify-write of `out`.
 // Only the 16-key groups that hold valid keys are multiplied (77 keys = 5 groups of the 8 staged; 4 / 16 image keys = 1 group).
-template <int D, int DP>
+template <int D, int DP, typename T>
 __global__ void __launch_bounds__(NTHR) attention_mma_shortk_kernel(fyc_attention_args a, int nqt) {
   constexpr int LDS = DP + 8;
   constexpr int KS = DP / 16;
   constexpr int NO = DP / 8;
   constexpr bool ONES = DP > D;
-  constexpr bool PACKED = DP > 80;                // D = 160: the first context's result waits as packed bf16 (register budget)
+  constexpr bool PACKED = DP > 80;                // D = 160: the first context's result waits as packed 16-bit pairs (register budget)
   extern __shared__ __align__(16) unsigned char smem_raw[];
-  bf16* sQ = reinterpret_cast<bf16*>(smem_raw);   // [2][64][LDS]
-  bf16* sK = sQ + 2 * 64 * LDS;                   // [3][64][LDS]  key tiles 0, 1 of the first context, tile 2 = second context
-  bf16* sV = sK + 3 * 64 * LDS;                   // [3][64][LDS]
+  T* sQ = reinterpret_cast<T*>(smem_raw);   // [2][64][LDS]
+  T* sK = sQ + 2 * 64 * LDS;                   // [3][64][LDS]  key tiles 0, 1 of the first context, tile 2 = second context
+  T* sV = sK + 3 * 64 * LDS;                   // [3][64][LDS]
   const int tid = threadIdx.x, lane = tid & 31, w = tid >> 5;
   const int g = lane >> 2, t = lane & 3;
   const int64_t n = blockIdx.z, h = blockIdx.y;
   const int64_t nk = n / a.kv_batch_div;
-  const bf16* qg = (const bf16*)a.q + n * a.bsq + h * D;
-  const bf16* kg = (const bf16*)a.k + nk * a.bsk + h * D;
-  const bf16* vg = (const bf16*)a.v + nk * a.bsv + h * D;
-  bf16* og = (bf16*)a.out + n * a.bso + h * D;
+  const T* qg = (const T*)a.q + n * a.bsq + h * D;
+  const T* kg = (const T*)a.k + nk * a.bsk + h * D;
+  const T* vg = (const T*)a.v + nk * a.bsv + h * D;
+  T* og = (T*)a.out + n * a.bso + h * D;
   const int nkt = (int)((a.Lk + BKV - 1) / BKV);  // 1 or 2
   const int npass = a.k2 ? 2 : 1;
   const float sl2 = a.scale * 1.4426950408889634f;
@@ -252,8 +243,8 @@ __global__ void __launch_bounds__(NTHR) attention_mma_shortk_kernel(fyc_attentio
     load_tile<D, DP, LDS, (DP > D)>(sV + kt * 64 * LDS, vg, a.ldv, (int64_t)kt * BKV, a.Lk, tid);
   }
   if (a.k2) {
-    load_tile<D, DP, LDS>(sK + 2 * 64 * LDS, (const bf16*)a.k2 + nk * a.bsk2 + h * D, a.ldk2, 0, a.Lk2, tid);
-    load_tile<D, DP, LDS, (DP > D)>(sV + 2 * 64 * LDS, (const bf16*)a.v2 + nk * a.bsv2 + h * D, a.ldv2, 0, a.Lk2, tid);
+    load_tile<D, DP, LDS>(sK + 2 * 64 * LDS, (const T*)a.k2 + nk * a.bsk2 + h * D, a.ldk2, 0, a.Lk2, tid);
+    load_tile<D, DP, LDS, (DP > D)>(sV + 2 * 64 * LDS, (const T*)a.v2 + nk * a.bsv2 + h * D, a.ldv2, 0, a.Lk2, tid);
   }
   int qt = blockIdx.x;
   if (qt < nqt) load_tile<D, DP, LDS>(sQ, qg, a.ldq, (int64_t)qt * BQ, a.Lq, tid);
@@ -276,7 +267,7 @@ __global__ void __launch_bounds__(NTHR) attention_mma_shortk_kernel(fyc_attentio
       ldmatrix_x4(qf[ks], sQ + qb * 64 * LDS + (w * 16 + (lane & 15)) * LDS + ks * 16 + (lane >> 4) * 8);
     float o[NO][4];
     float accf[PACKED ? 1 : NO][4];                 // first context's finished result (fp32), or ...
-    uint32_t accp[PACKED ? NO : 1][2];              // ... packed bf16 pairs (rows g, g+8)
+    uint32_t accp[PACKED ? NO : 1][2];              // ... packed 16-bit pairs (rows g, g+8)
 
 #pragma unroll 1
     for (int pass = 0; pass < npass; ++pass) {
@@ -287,8 +278,8 @@ __global__ void __launch_bounds__(NTHR) attention_mma_shortk_kernel(fyc_attentio
       float m0 = -INFINITY, m1 = -INFINITY, l0 = 0.f, l1 = 0.f;
 
       for (int kt = 0; kt < ntl; ++kt) {
-        const bf16* kb = sK + (tile0 + kt) * 64 * LDS;
-        const bf16* vb = sV + (tile0 + kt) * 64 * LDS;
+        const T* kb = sK + (tile0 + kt) * 64 * LDS;
+        const T* vb = sV + (tile0 + kt) * 64 * LDS;
         const int nvalid = (int)min((int64_t)BKV, Lp - (int64_t)kt * BKV);     // valid keys of this tile (>= 1)
         const int ngrp = (nvalid + 15) >> 4;                                    // 16-key groups that hold any
         float s[8][4];
@@ -302,8 +293,8 @@ __global__ void __launch_bounds__(NTHR) attention_mma_shortk_kernel(fyc_attentio
               uint32_t b[4];
               const int mi = lane >> 3;
               ldmatrix_x4(b, kb + (jp * 16 + (lane & 7) + (mi >> 1) * 8) * LDS + ks * 16 + (mi & 1) * 8);
-              mma_bf16(s[2 * jp], qf[ks], b[0], b[1]);
-              mma_bf16(s[2 * jp + 1], qf[ks], b[2], b[3]);
+              mma16816<T>(s[2 * jp], qf[ks], b[0], b[1]);
+              mma16816<T>(s[2 * jp + 1], qf[ks], b[2], b[3]);
             }
           }
         }
@@ -334,8 +325,8 @@ __global__ void __launch_bounds__(NTHR) attention_mma_shortk_kernel(fyc_attentio
             float p0 = ex2_approx(fmaf(s[j][0], sl2, nb0)), p1 = ex2_approx(fmaf(s[j][1], sl2, nb0));
             float p2 = ex2_approx(fmaf(s[j][2], sl2, nb1)), p3 = ex2_approx(fmaf(s[j][3], sl2, nb1));
             if constexpr (!ONES) { rs0 += p0 + p1; rs1 += p2 + p3; }
-            pf[j >> 1][(j & 1) * 2 + 0] = pack_bf16(p0, p1);
-            pf[j >> 1][(j & 1) * 2 + 1] = pack_bf16(p2, p3);
+            pf[j >> 1][(j & 1) * 2 + 0] = pack_u32<T>(p0, p1);
+            pf[j >> 1][(j & 1) * 2 + 1] = pack_u32<T>(p2, p3);
           }
         }
         if constexpr (!ONES) {
@@ -355,8 +346,8 @@ __global__ void __launch_bounds__(NTHR) attention_mma_shortk_kernel(fyc_attentio
               uint32_t b[4];
               const int mi = lane >> 3;
               ldmatrix_x4_trans(b, vb + (kk * 16 + (lane & 7) + (mi & 1) * 8) * LDS + np * 16 + (mi >> 1) * 8);
-              mma_bf16(o[2 * np], pf[kk], b[0], b[1]);
-              mma_bf16(o[2 * np + 1], pf[kk], b[2], b[3]);
+              mma16816<T>(o[2 * np], pf[kk], b[0], b[1]);
+              mma16816<T>(o[2 * np + 1], pf[kk], b[2], b[3]);
             }
           }
         }
@@ -371,7 +362,7 @@ __global__ void __launch_bounds__(NTHR) attention_mma_shortk_kernel(fyc_attentio
       if (pass == 0 && npass == 2) {                 // park  out_alpha * softmax(q K_t^T) V_t  while the image keys are processed
 #pragma unroll
         for (int i = 0; i < NO; ++i) {
-          if constexpr (PACKED) { accp[i][0] = pack_bf16(o[i][0] * i0, o[i][1] * i0); accp[i][1] = pack_bf16(o[i][2] * i1, o[i][3] * i1); }
+          if constexpr (PACKED) { accp[i][0] = pack_u32<T>(o[i][0] * i0, o[i][1] * i0); accp[i][1] = pack_u32<T>(o[i][2] * i1, o[i][3] * i1); }
           else { accf[i][0] = o[i][0] * i0; accf[i][1] = o[i][1] * i0; accf[i][2] = o[i][2] * i1; accf[i][3] = o[i][3] * i1; }
         }
       } else {
@@ -380,8 +371,8 @@ __global__ void __launch_bounds__(NTHR) attention_mma_shortk_kernel(fyc_attentio
           o[i][0] *= i0; o[i][1] *= i0; o[i][2] *= i1; o[i][3] *= i1;
           if (pass == 1) {
             if constexpr (PACKED) {
-              const float2 e0 = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&accp[i][0]));
-              const float2 e1 = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&accp[i][1]));
+              const float2 e0 = Pair16<T>::unpack(*reinterpret_cast<const typename Pair16<T>::type*>(&accp[i][0]));
+              const float2 e1 = Pair16<T>::unpack(*reinterpret_cast<const typename Pair16<T>::type*>(&accp[i][1]));
               o[i][0] += e0.x; o[i][1] += e0.y; o[i][2] += e1.x; o[i][3] += e1.y;
             } else { o[i][0] += accf[i][0]; o[i][1] += accf[i][1]; o[i][2] += accf[i][2]; o[i][3] += accf[i][3]; }
           }
@@ -394,16 +385,16 @@ __global__ void __launch_bounds__(NTHR) attention_mma_shortk_kernel(fyc_attentio
       const int col = i * 8 + 2 * t;
       if (col < D) {
         if (r0 < a.Lq) {
-          __nv_bfloat162* dst = reinterpret_cast<__nv_bfloat162*>(og + r0 * a.ldo + col);
+          typename Pair16<T>::type* dst = reinterpret_cast<typename Pair16<T>::type*>(og + r0 * a.ldo + col);
           float x = o[i][0], y = o[i][1];
-          if (a.accumulate) { float2 e = __bfloat1622float2(*dst); x += e.x; y += e.y; }
-          *dst = __floats2bfloat162_rn(x, y);
+          if (a.accumulate) { float2 e = Pair16<T>::unpack(*dst); x += e.x; y += e.y; }
+          *dst = Pair16<T>::pack(x, y);
         }
         if (r1 < a.Lq) {
-          __nv_bfloat162* dst = reinterpret_cast<__nv_bfloat162*>(og + r1 * a.ldo + col);
+          typename Pair16<T>::type* dst = reinterpret_cast<typename Pair16<T>::type*>(og + r1 * a.ldo + col);
           float x = o[i][2], y = o[i][3];
-          if (a.accumulate) { float2 e = __bfloat1622float2(*dst); x += e.x; y += e.y; }
-          *dst = __floats2bfloat162_rn(x, y);
+          if (a.accumulate) { float2 e = Pair16<T>::unpack(*dst); x += e.x; y += e.y; }
+          *dst = Pair16<T>::pack(x, y);
         }
       }
     }
@@ -416,11 +407,11 @@ static bool shortk_enabled() {
   return !(e && e[0] == '0');
 }
 
-template <int D, int DP>
+template <int D, int DP, typename T>
 int32_t launch_mma_shortk(const fyc_attention_args* a, cudaStream_t st) {
   constexpr int LDS = DP + 8;
-  const size_t smem = (size_t)8 * 64 * LDS * sizeof(bf16);     // 2 Q + 3 K + 3 V tiles
-  auto kern = attention_mma_shortk_kernel<D, DP>;
+  const size_t smem = (size_t)8 * 64 * LDS * sizeof(T);     // 2 Q + 3 K + 3 V tiles
+  auto kern = attention_mma_shortk_kernel<D, DP, T>;
   FYC_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   const int nqt = (int)ceil_div64(a->Lq, BQ);
   // CTAs per (image, head): enough to fill the machine (~227 KB of shared memory per SM), at most one per query tile
@@ -435,21 +426,21 @@ int32_t launch_mma_shortk(const fyc_attention_args* a, cudaStream_t st) {
   return FYC_OK;
 }
 
-template <int D, int DP>
+template <int D, int DP, typename T>
 int32_t launch_mma(const fyc_attention_args* a, cudaStream_t st) {
   if (a->k2) {     // fused two-context form (IP cross-attention): one launch when both contexts fit the resident kernel, else two passes
-    if (a->Lk <= 2 * BKV && a->Lk2 <= BKV) return launch_mma_shortk<D, DP>(a, st);
+    if (a->Lk <= 2 * BKV && a->Lk2 <= BKV) return launch_mma_shortk<D, DP, T>(a, st);
     fyc_attention_args p1 = *a, p2 = *a;
     p1.k2 = p1.v2 = nullptr;
     p2.k = a->k2; p2.v = a->v2; p2.Lk = a->Lk2; p2.ldk = a->ldk2; p2.ldv = a->ldv2; p2.bsk = a->bsk2; p2.bsv = a->bsv2;
     p2.k2 = p2.v2 = nullptr; p2.out_alpha = a->alpha2; p2.accumulate = 1;
-    const int32_t rc = launch_mma<D, DP>(&p1, st);
-    return rc ? rc : launch_mma<D, DP>(&p2, st);
+    const int32_t rc = launch_mma<D, DP, T>(&p1, st);
+    return rc ? rc : launch_mma<D, DP, T>(&p2, st);
   }
-  if (a->Lk <= 2 * BKV && a->Lq >= 4 * BQ && DP <= 80 && shortk_enabled()) return launch_mma_shortk<D, DP>(a, st);
+  if (a->Lk <= 2 * BKV && a->Lq >= 4 * BQ && DP <= 80 && shortk_enabled()) return launch_mma_shortk<D, DP, T>(a, st);
   constexpr int LDS = DP + 8;
-  const size_t smem = (size_t)5 * 64 * LDS * sizeof(bf16);
-  auto kern = attention_mma_kernel<D, DP>;
+  const size_t smem = (size_t)5 * 64 * LDS * sizeof(T);
+  auto kern = attention_mma_kernel<D, DP, T>;
   FYC_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   dim3 grid((unsigned)ceil_div64(a->Lq, BQ), (unsigned)a->heads, (unsigned)a->batch);
   kern<<<grid, NTHR, smem, st>>>(*a);
@@ -460,7 +451,7 @@ int32_t launch_mma(const fyc_attention_args* a, cudaStream_t st) {
 }  // namespace
 
 bool fyc_attention_mma_eligible(const fyc_attention_args* a) {
-  if (a->dtype != FYC_BF16) return false;
+  if (!fyc_is_16bit(a->dtype)) return false;
   if (a->D != 40 && a->D != 80 && a->D != 160 && a->D != 64) return false;
   if ((a->ldq | a->ldk | a->ldv | a->bsq | a->bsk | a->bsv) % 8) return false;
   if ((a->ldo | a->bso) % 2) return false;
@@ -472,11 +463,11 @@ bool fyc_attention_mma_eligible(const fyc_attention_args* a) {
 }
 
 int32_t fyc_attention_mma(const fyc_attention_args* a, cudaStream_t st) {
-  switch (a->D) {
-    case 40: return launch_mma<40, 48>(a, st);
-    case 64: return launch_mma<64, 64>(a, st);
-    case 80: return launch_mma<80, 80>(a, st);
-    case 160: return launch_mma<160, 160>(a, st);
-  }
+  FYC_DISPATCH16(a->dtype, switch (a->D) {
+    case 40: return launch_mma<40, 48, T>(a, st);
+    case 64: return launch_mma<64, 64, T>(a, st);
+    case 80: return launch_mma<80, 80, T>(a, st);
+    case 160: return launch_mma<160, 160, T>(a, st);
+  })
   FYC_CHECK(false, "attention(mma): unsupported head dim %lld", (long long)a->D);
 }

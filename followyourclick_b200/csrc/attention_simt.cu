@@ -149,7 +149,7 @@ __global__ void __launch_bounds__(256) temporal_attention_kernel(const T* __rest
   const int64_t p = bp % HW, b = bp / HW;
   const int64_t row_stride = HW * 3 * C;                     // frame stride in the qkv tensor
   const T* src = qkv + (b * F * HW + p) * 3 * C + h * D;
-  // cooperative load: 3 segments x F rows x D elements, 4-element (8 B bf16 / 16 B fp32) vectors
+  // cooperative load: 3 segments x F rows x D elements, 4-element (8 B bf16 / fp16, 16 B fp32) vectors
   const int dv = D / 4;
   for (int i = lane; i < 3 * F * dv; i += 32) {
     int seg = i / (F * dv);
@@ -239,20 +239,21 @@ int32_t fyc_attention_simt(const fyc_attention_args* a, cudaStream_t st) {
   return launch_attn<T, 8>(a, st);
   if (a->dtype == FYC_F32) { FYC_ATTN_DI(float) }
   if (a->dtype == FYC_BF16) { FYC_ATTN_DI(bf16) }
+  if (a->dtype == FYC_F16) { FYC_ATTN_DI(f16) }
 #undef FYC_ATTN_DI
   FYC_CHECK(false, "attention: unknown dtype %d", a->dtype);
 }
 
 bool fyc_temporal_mma_eligible(int64_t F, int64_t D, int64_t heads, int32_t dtype, const void* qkv, const void* out);
 int32_t fyc_temporal_attention_mma(const void* qkv, void* out, int64_t B, int64_t F, int64_t HW, int64_t heads, int64_t D, float scale,
-                                   cudaStream_t st);
+                                   int32_t dtype, cudaStream_t st);
 
 extern "C" int32_t fyc_temporal_attention(const void* qkv, void* out, int64_t B, int64_t F, int64_t HW, int64_t heads,
                                           int64_t D, float scale, int32_t dtype, void* stream) {
   cudaStream_t st = (cudaStream_t)stream;
   FYC_CHECK(F >= 1 && F <= 32, "temporal_attention: F=%lld must be in [1, 32]", (long long)F);
   FYC_CHECK(D % 4 == 0, "temporal_attention: head dim %lld must be a multiple of 4", (long long)D);
-  if (fyc_temporal_mma_eligible(F, D, heads, dtype, qkv, out)) return fyc_temporal_attention_mma(qkv, out, B, F, HW, heads, D, scale, st);
+  if (fyc_temporal_mma_eligible(F, D, heads, dtype, qkv, out)) return fyc_temporal_attention_mma(qkv, out, B, F, HW, heads, D, scale, dtype, st);
 #define FYC_TA(T)                                                                                             \
   if (F <= 4) return launch_temporal<T, 4>((const T*)qkv, (T*)out, B, (int)F, HW, (int)heads, (int)D, scale, st);   \
   if (F <= 8) return launch_temporal<T, 8>((const T*)qkv, (T*)out, B, (int)F, HW, (int)heads, (int)D, scale, st);   \
@@ -260,6 +261,7 @@ extern "C" int32_t fyc_temporal_attention(const void* qkv, void* out, int64_t B,
   return launch_temporal<T, 32>((const T*)qkv, (T*)out, B, (int)F, HW, (int)heads, (int)D, scale, st);
   if (dtype == FYC_F32) { FYC_TA(float) }
   if (dtype == FYC_BF16) { FYC_TA(bf16) }
+  if (dtype == FYC_F16) { FYC_TA(f16) }
 #undef FYC_TA
   FYC_CHECK(false, "temporal_attention: unknown dtype %d", dtype);
 }

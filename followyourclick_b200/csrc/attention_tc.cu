@@ -67,10 +67,6 @@ __device__ __forceinline__ float ex2(float x) {
   asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
   return y;
 }
-__device__ __forceinline__ uint32_t pack_bf16(float lo, float hi) {
-  __nv_bfloat162 v = __floats2bfloat162_rn(lo, hi);
-  return *reinterpret_cast<uint32_t*>(&v);
-}
 __device__ __forceinline__ float quad_max(float v) {
   v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, 1));
   return fmaxf(v, __shfl_xor_sync(0xffffffffu, v, 2));
@@ -79,34 +75,37 @@ __device__ __forceinline__ float quad_sum(float v) {
   v += __shfl_xor_sync(0xffffffffu, v, 1);
   return v + __shfl_xor_sync(0xffffffffu, v, 2);
 }
-// register accumulator of n-tiles [2 kk, 2 kk + 1] (rows r, r + 8) -> the A fragment of k-step kk
+// register accumulator of n-tiles [2 kk, 2 kk + 1] (rows r, r + 8) -> the A fragment of k-step kk, as pairs of T
+template <typename T>
 __device__ __forceinline__ void pack_a(const float* p, int kk, uint32_t* a) {
-  a[0] = pack_bf16(p[8 * kk + 0], p[8 * kk + 1]);
-  a[1] = pack_bf16(p[8 * kk + 2], p[8 * kk + 3]);
-  a[2] = pack_bf16(p[8 * kk + 4], p[8 * kk + 5]);
-  a[3] = pack_bf16(p[8 * kk + 6], p[8 * kk + 7]);
+  a[0] = pack_u32<T>(p[8 * kk + 0], p[8 * kk + 1]);
+  a[1] = pack_u32<T>(p[8 * kk + 2], p[8 * kk + 3]);
+  a[2] = pack_u32<T>(p[8 * kk + 4], p[8 * kk + 5]);
+  a[3] = pack_u32<T>(p[8 * kk + 6], p[8 * kk + 7]);
 }
 // out[row, col .. col + 1] for the n-tiles of a 64 x DV accumulator that hold real columns (< D)
-template <int DV, int D>
-__device__ __forceinline__ void store_rows(bf16* og, int64_t ldo, int64_t r0, int64_t nrows, const float* o, float s0, float s1, int q) {
+template <int DV, int D, typename T>
+__device__ __forceinline__ void store_rows(T* og, int64_t ldo, int64_t r0, int64_t nrows, const float* o, float s0, float s1, int q) {
+  typedef typename Pair16<T>::type P;
 #pragma unroll
   for (int j = 0; j < DV / 8; ++j) {
     const int col = 8 * j + 2 * q;
     if (col >= D) continue;
-    if (r0 < nrows) *reinterpret_cast<__nv_bfloat162*>(og + r0 * ldo + col) = __floats2bfloat162_rn(o[4 * j] * s0, o[4 * j + 1] * s0);
-    if (r0 + 8 < nrows) *reinterpret_cast<__nv_bfloat162*>(og + (r0 + 8) * ldo + col) = __floats2bfloat162_rn(o[4 * j + 2] * s1, o[4 * j + 3] * s1);
+    if (r0 < nrows) *reinterpret_cast<P*>(og + r0 * ldo + col) = Pair16<T>::pack(o[4 * j] * s0, o[4 * j + 1] * s0);
+    if (r0 + 8 < nrows) *reinterpret_cast<P*>(og + (r0 + 8) * ldo + col) = Pair16<T>::pack(o[4 * j + 2] * s1, o[4 * j + 3] * s1);
   }
 }
 
 struct AttnTcParams {
-  bf16* out; int64_t ldo, bso;      // out[n, token, h*D + d]
+  void* out; int64_t ldo, bso;      // out[n, token, h*D + d]
   int L, heads;
   float scale_log2e;
 };
 
 // KA: 64-column atoms per q / k head (1: D = 40 zero-padded to 64 or D = 64, 2: D = 80), KS: k-steps of QK^T that hold data, DV: PV accumulator
-// columns (D rounded up to a multiple of 16 rows of V^T; the extra rows belong to the next head and only feed unstored columns)
-template <int KA, int KS, int DV, int D>
+// columns (D rounded up to a multiple of 16 rows of V^T; the extra rows belong to the next head and only feed unstored columns); T: the
+// 16-bit operand / output type (bf16 | f16)
+template <int KA, int KS, int DV, int D, typename T>
 __global__ void __launch_bounds__(NTHREADS, 1)
 attention_tc_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant__ CUtensorMap map_k, const __grid_constant__ CUtensorMap map_v,
                     const AttnTcParams p) {
@@ -155,7 +154,7 @@ attention_tc_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_cons
     wgmma_fence();
 #pragma unroll
     for (int ks = 0; ks < KS; ++ks)
-      Wgmma<BKV>::ss(sc, wgmma_desc_sw128(sq + (ks >> 2) * ATOM_BYTES) + 2 * (ks & 3), wgmma_desc_sw128(sk + (ks >> 2) * ATOM_BYTES) + 2 * (ks & 3),
+      Wgmma<BKV, T>::ss(sc, wgmma_desc_sw128(sq + (ks >> 2) * ATOM_BYTES) + 2 * (ks & 3), wgmma_desc_sw128(sk + (ks >> 2) * ATOM_BYTES) + 2 * (ks & 3),
                      ks > 0 ? 1 : 0);
     wgmma_commit();
     wgmma_wait<0>();
@@ -182,10 +181,10 @@ attention_tc_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_cons
     for (int t = 0; t < DV / 8; ++t) { o[4 * t] *= c0; o[4 * t + 1] *= c0; o[4 * t + 2] *= c1; o[4 * t + 3] *= c1; }
     uint32_t pa[BKV / 16][4];
 #pragma unroll
-    for (int kk = 0; kk < BKV / 16; ++kk) pack_a(sc, kk, pa[kk]);
+    for (int kk = 0; kk < BKV / 16; ++kk) pack_a<T>(sc, kk, pa[kk]);
     wgmma_fence();
 #pragma unroll
-    for (int kk = 0; kk < BKV / 16; ++kk) Wgmma<DV>::rs(o, pa[kk], wgmma_desc_sw128(sv + (kk >> 2) * VBOX) + 2 * (kk & 3), 1);
+    for (int kk = 0; kk < BKV / 16; ++kk) Wgmma<DV, T>::rs(o, pa[kk], wgmma_desc_sw128(sv + (kk >> 2) * VBOX) + 2 * (kk & 3), 1);
     wgmma_commit();
     wgmma_wait<0>();
     wgmma_fence_regs<DV / 2>(o);
@@ -193,14 +192,14 @@ attention_tc_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_cons
     if (threadIdx.x == 0 && j + 2 < nkv) load_kv(j + 2);
   }
   l0 = quad_sum(l0); l1 = quad_sum(l1);
-  bf16* og = p.out + (int64_t)n * p.bso + (int64_t)h * D;
+  T* og = (T*)p.out + (int64_t)n * p.bso + (int64_t)h * D;
   const int64_t r0 = q0 + wg * 64 + (warp & 3) * 16 + (lane >> 2);
-  store_rows<DV, D>(og, p.ldo, r0, p.L, o, 1.0f / l0, 1.0f / l1, q);
+  store_rows<DV, D, T>(og, p.ldo, r0, p.L, o, 1.0f / l0, 1.0f / l1, q);
 }
 
 // ------------------------------------------------------------------------------------------------------------------------------
 struct AttnCxParams {
-  bf16* out; int64_t ldo, bso;
+  void* out; int64_t ldo, bso;
   int Lq, heads, Lk, Lk2, kv_div, nqt;
   float scale_log2e, out_alpha, alpha2;
 };
@@ -231,7 +230,7 @@ __device__ __forceinline__ void softmax_ctx(float* sc, int Lk, float wgt, float 
   for (int t = 0; t < NT; ++t) { sc[4 * t] *= f0; sc[4 * t + 1] *= f0; sc[4 * t + 2] *= f1; sc[4 * t + 3] *= f1; }
 }
 
-template <int KA, int KS, int DV, int D>
+template <int KA, int KS, int DV, int D, typename T>
 __global__ void __launch_bounds__(NTHREADS, 1)
 attention_cx_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant__ CUtensorMap map_k, const __grid_constant__ CUtensorMap map_v,
                     const __grid_constant__ CUtensorMap map_k2, const __grid_constant__ CUtensorMap map_v2, const AttnCxParams p) {
@@ -274,7 +273,7 @@ attention_cx_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_cons
   mbar_wait(cbar, 0);
   const float sl2 = p.scale_log2e;
   const uint32_t skt = smem_u32(smem + OFF_KT), svt = smem_u32(smem + OFF_VT), ski = smem_u32(smem + OFF_KI), svi = smem_u32(smem + OFF_VI);
-  bf16* og = p.out + (int64_t)n * p.bso + (int64_t)h * D;
+  T* og = (T*)p.out + (int64_t)n * p.bso + (int64_t)h * D;
   for (int it = 0, qt = blockIdx.x; qt < p.nqt; ++it, qt += gridDim.x) {
     mbar_wait(&qfull[it & 1], (uint32_t)(it >> 1) & 1u);
     const uint32_t sq = smem_u32(smem + (it & 1) * Q_BYTES) + (uint32_t)wg * (64 * 128);
@@ -282,12 +281,12 @@ attention_cx_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_cons
     wgmma_fence();
 #pragma unroll
     for (int ks = 0; ks < KS; ++ks)
-      Wgmma<CX_LK>::ss(st, wgmma_desc_sw128(sq + (ks >> 2) * ATOM_BYTES) + 2 * (ks & 3), wgmma_desc_sw128(skt + (ks >> 2) * KT_ATOM) + 2 * (ks & 3),
+      Wgmma<CX_LK, T>::ss(st, wgmma_desc_sw128(sq + (ks >> 2) * ATOM_BYTES) + 2 * (ks & 3), wgmma_desc_sw128(skt + (ks >> 2) * KT_ATOM) + 2 * (ks & 3),
                        ks > 0 ? 1 : 0);
     if (two) {
 #pragma unroll
       for (int ks = 0; ks < KS; ++ks)
-        Wgmma<CX_LK2>::ss(si, wgmma_desc_sw128(sq + (ks >> 2) * ATOM_BYTES) + 2 * (ks & 3), wgmma_desc_sw128(ski + (ks >> 2) * KI_ATOM) + 2 * (ks & 3),
+        Wgmma<CX_LK2, T>::ss(si, wgmma_desc_sw128(sq + (ks >> 2) * ATOM_BYTES) + 2 * (ks & 3), wgmma_desc_sw128(ski + (ks >> 2) * KI_ATOM) + 2 * (ks & 3),
                           ks > 0 ? 1 : 0);
     }
     wgmma_commit();
@@ -298,18 +297,18 @@ attention_cx_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_cons
     if (two) softmax_ctx<CX_LK2 / 8>(si, p.Lk2, p.alpha2, sl2, q);
     uint32_t pt[CX_LK / 16][4], pi[4];
 #pragma unroll
-    for (int kk = 0; kk < CX_LK / 16; ++kk) pack_a(st, kk, pt[kk]);
-    pack_a(si, 0, pi);
+    for (int kk = 0; kk < CX_LK / 16; ++kk) pack_a<T>(st, kk, pt[kk]);
+    pack_a<T>(si, 0, pi);
     float o[DV / 2];
     wgmma_fence();
 #pragma unroll
-    for (int kk = 0; kk < CX_LK / 16; ++kk) Wgmma<DV>::rs(o, pt[kk], wgmma_desc_sw128(svt + (kk >> 2) * VBOX) + 2 * (kk & 3), kk > 0 ? 1 : 0);
-    if (two) Wgmma<DV>::rs(o, pi, wgmma_desc_sw128(svi), 1);
+    for (int kk = 0; kk < CX_LK / 16; ++kk) Wgmma<DV, T>::rs(o, pt[kk], wgmma_desc_sw128(svt + (kk >> 2) * VBOX) + 2 * (kk & 3), kk > 0 ? 1 : 0);
+    if (two) Wgmma<DV, T>::rs(o, pi, wgmma_desc_sw128(svi), 1);
     wgmma_commit();
     wgmma_wait<0>();
     wgmma_fence_regs<DV / 2>(o);
     const int64_t r0 = (int64_t)qt * BQ + wg * 64 + (warp & 3) * 16 + (lane >> 2);
-    store_rows<DV, D>(og, p.ldo, r0, p.Lq, o, 1.0f, 1.0f, q);
+    store_rows<DV, D, T>(og, p.ldo, r0, p.Lq, o, 1.0f, 1.0f, q);
     __syncthreads();                                 // both warpgroups are done with this Q buffer
     if (threadIdx.x == 0 && qt + 2 * (int)gridDim.x < p.nqt) load_q(it + 2);
   }
@@ -318,7 +317,8 @@ attention_cx_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_cons
 template <int KA, int KS, int DV, int D> constexpr int self_smem() { return KA * ATOM_BYTES + 2 * (KA * ATOM_BYTES + 2 * DV * 128) + 64 + 1024; }
 template <int KA, int DV> constexpr int cx_smem() { return 2 * KA * ATOM_BYTES + KA * CX_LK * 128 + 2 * DV * 128 + KA * CX_LK2 * 128 + DV * 128 + 64 + 1024; }
 
-// [NB, L, ld] (columns col0 .. col0+C) -> [NB, C, L]   (V -> V^T so that keys are the contiguous, K-major dimension of PV)
+// [NB, L, ld] (columns col0 .. col0+C) -> [NB, C, L]   (V -> V^T so that keys are the contiguous, K-major dimension of PV).  It only moves
+// 16-bit values, so it serves bf16 and fp16 alike.
 __global__ void __launch_bounds__(256) transpose_tokens_kernel(const bf16* __restrict__ in, bf16* __restrict__ out, int L, int C,
                                                                int64_t ld, int64_t col0) {
   __shared__ bf16 tile[64][66];
@@ -359,26 +359,38 @@ EncodeTiledFn encode_fn() {
   }
   return fn;
 }
-int32_t make_map(CUtensorMap* m, const void* base, int rank, const uint64_t* dims, const uint64_t* strides, const uint32_t* box) {
+int32_t make_map(CUtensorMap* m, const void* base, int rank, const uint64_t* dims, const uint64_t* strides, const uint32_t* box, int32_t dt) {
   EncodeTiledFn fn = encode_fn();
   FYC_CHECK(fn != nullptr, "attention(tensor cores): cuTensorMapEncodeTiled unavailable");
   cuuint64_t gd[5], gs[4]; cuuint32_t bx[5], es[5];
   for (int i = 0; i < rank; ++i) { gd[i] = dims[i]; bx[i] = box[i]; es[i] = 1; }
   for (int i = 0; i + 1 < rank; ++i) gs[i] = strides[i];
-  CUresult r = fn(m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, (cuuint32_t)rank, const_cast<void*>(base), gd, gs, bx, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
+  CUresult r = fn(m, dt == FYC_F16 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, (cuuint32_t)rank, const_cast<void*>(base), gd, gs, bx, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
                   CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   FYC_CHECK(r == CUDA_SUCCESS, "attention(tensor cores): cuTensorMapEncodeTiled failed (%d)", (int)r);
   return FYC_OK;
 }
 
-template <int KA, int KS, int DV, int D>
+template <int KA, int KS, int DV, int D, typename T>
 int32_t launch_self(const CUtensorMap& mq, const CUtensorMap& mk, const CUtensorMap& mv, const AttnTcParams& p, int64_t NB, cudaStream_t st) {
   constexpr int smem = self_smem<KA, KS, DV, D>();
-  auto kern = attention_tc_kernel<KA, KS, DV, D>;
+  auto kern = attention_tc_kernel<KA, KS, DV, D, T>;
   static bool attr = false;
   if (!attr) { FYC_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem)); attr = true; }
   dim3 grid((unsigned)(p.L / BQ), (unsigned)p.heads, (unsigned)NB);
   kern<<<grid, NTHREADS, smem, st>>>(mq, mk, mv, p);
+  FYC_LAUNCH_CHECK();
+  return FYC_OK;
+}
+
+template <int KA, int KS, int DV, int D, typename T>
+int32_t launch_cx(const CUtensorMap& mq, const CUtensorMap& mk, const CUtensorMap& mv, const CUtensorMap& mk2, const CUtensorMap& mv2,
+                  const AttnCxParams& p, dim3 grid, cudaStream_t st) {
+  constexpr int smem = cx_smem<KA, DV>();
+  auto kern = attention_cx_kernel<KA, KS, DV, D, T>;
+  static bool attr = false;
+  if (!attr) { FYC_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem)); attr = true; }
+  kern<<<grid, NTHREADS, smem, st>>>(mq, mk, mv, mk2, mv2, p);
   FYC_LAUNCH_CHECK();
   return FYC_OK;
 }
@@ -394,9 +406,9 @@ extern "C" int32_t fyc_transpose_tokens(const void* in, void* out, int64_t NB, i
   return FYC_OK;
 }
 
-// qk: [NB, L, ldqk] bf16 with q head h at columns [q_col0 + 64h, +64) and k head h at [k_col0 + 64h, +64) (D = 40: cols 40..63 zero;
+// qk: [NB, L, ldqk] 16-bit (dt) with q head h at columns [q_col0 + 64h, +64) and k head h at [k_col0 + 64h, +64) (D = 40: cols 40..63 zero;
 // D = 64: the unpadded fused projection); vt: [NB, heads*D, L]; out: [NB, L, ldo] (head h at columns [h*D, (h+1)*D)).
-extern "C" int32_t fyc_self_attention_tc(const void* qk, int64_t ldqk, int64_t q_col0, int64_t k_col0, const void* vt, void* out,
+static int32_t self_attention_tc(int32_t dt, const void* qk, int64_t ldqk, int64_t q_col0, int64_t k_col0, const void* vt, void* out,
                                          int64_t ldo, int64_t NB, int64_t heads, int64_t L, int64_t D, float scale, void* stream) {
   FYC_CHECK(D == 40 || D == 64, "self_attention_tc: built for head dims 40 and 64 (got %lld)", (long long)D);
   FYC_CHECK(L % 128 == 0 && L >= 128, "self_attention_tc: sequence length %lld must be a multiple of 128", (long long)L);
@@ -408,29 +420,32 @@ extern "C" int32_t fyc_self_attention_tc(const void* qk, int64_t ldqk, int64_t q
     uint64_t dims[4] = {64, (uint64_t)L, (uint64_t)heads, (uint64_t)NB};
     uint64_t str[3] = {(uint64_t)ldqk * 2, 128, (uint64_t)L * ldqk * 2};
     uint32_t box[4] = {64, (uint32_t)BQ, 1, 1};
-    int32_t rc = make_map(&mq, (const bf16*)qk + q_col0, 4, dims, str, box);
+    int32_t rc = make_map(&mq, (const uint16_t*)qk + q_col0, 4, dims, str, box, dt);
     if (rc) return rc;
-    rc = make_map(&mk, (const bf16*)qk + k_col0, 4, dims, str, box);
+    rc = make_map(&mk, (const uint16_t*)qk + k_col0, 4, dims, str, box, dt);
     if (rc) return rc;
   }
   {
     uint64_t dims[3] = {(uint64_t)L, (uint64_t)(heads * D), (uint64_t)NB};
     uint64_t str[2] = {(uint64_t)L * 2, (uint64_t)L * heads * D * 2};
     uint32_t box[3] = {64, D == 40 ? 48u : 64u, 1};
-    int32_t rc = make_map(&mv, vt, 3, dims, str, box);
+    int32_t rc = make_map(&mv, vt, 3, dims, str, box, dt);
     if (rc) return rc;
   }
   AttnTcParams p;
-  p.out = (bf16*)out; p.ldo = ldo; p.bso = L * ldo; p.L = (int)L; p.heads = (int)heads;
+  p.out = out; p.ldo = ldo; p.bso = L * ldo; p.L = (int)L; p.heads = (int)heads;
   p.scale_log2e = scale * 1.4426950408889634f;
-  if (D == 64) return launch_self<1, 4, 64, 64>(mq, mk, mv, p, NB, (cudaStream_t)stream);
-  return launch_self<1, 3, 48, 40>(mq, mk, mv, p, NB, (cudaStream_t)stream);      // k-step 3 would multiply the zero columns 48..63
+  FYC_DISPATCH16(dt, {
+    if (D == 64) return launch_self<1, 4, 64, 64, T>(mq, mk, mv, p, NB, (cudaStream_t)stream);
+    return launch_self<1, 3, 48, 40, T>(mq, mk, mv, p, NB, (cudaStream_t)stream);      // k-step 3 would multiply the zero columns 48..63
+  })
+  return FYC_OK;
 }
 
-// Head dim 80 (level-1 self-attention): qkv [NB, L, ldqkv] bf16 with q head h at columns [q_col0 + 80 h, +80), k at [k_col0 + 80 h, +80) -
+// Head dim 80 (level-1 self-attention): qkv [NB, L, ldqkv] 16-bit (dt) with q head h at columns [q_col0 + 80 h, +80), k at [k_col0 + 80 h, +80) -
 // UNPADDED, the fused [q | k | v] projection as the GEMM wrote it (reads up to column k_col0 + 80 heads + 47: the buffer must hold at
 // least 48 more columns after k's last head, which the v block provides); vt: [NB, heads * 80, L]; out: [NB, L, ldo].
-extern "C" int32_t fyc_self_attention_tc_d80(const void* qkv, int64_t ldqkv, int64_t q_col0, int64_t k_col0, const void* vt, void* out,
+static int32_t self_attention_tc_d80(int32_t dt, const void* qkv, int64_t ldqkv, int64_t q_col0, int64_t k_col0, const void* vt, void* out,
                                              int64_t ldo, int64_t NB, int64_t heads, int64_t L, float scale, void* stream) {
   constexpr int D = 80;
   FYC_CHECK(L % (2 * BQ) == 0 && L >= 2 * BQ, "self_attention_tc_d80: sequence length %lld must be a multiple of 256", (long long)L);
@@ -445,30 +460,31 @@ extern "C" int32_t fyc_self_attention_tc_d80(const void* qkv, int64_t ldqkv, int
     uint64_t dims[4] = {128, (uint64_t)L, (uint64_t)heads, (uint64_t)NB};
     uint64_t str[3] = {(uint64_t)ldqkv * 2, (uint64_t)D * 2, (uint64_t)L * ldqkv * 2};
     uint32_t box[4] = {64, (uint32_t)BQ, 1, 1};
-    int32_t rc = make_map(&mq, (const bf16*)qkv + q_col0, 4, dims, str, box);
+    int32_t rc = make_map(&mq, (const uint16_t*)qkv + q_col0, 4, dims, str, box, dt);
     if (rc) return rc;
-    rc = make_map(&mk, (const bf16*)qkv + k_col0, 4, dims, str, box);
+    rc = make_map(&mk, (const uint16_t*)qkv + k_col0, 4, dims, str, box, dt);
     if (rc) return rc;
   }
   {
     uint64_t dims[3] = {(uint64_t)L, (uint64_t)(heads * D), (uint64_t)NB};
     uint64_t str[2] = {(uint64_t)L * 2, (uint64_t)L * heads * D * 2};
     uint32_t box[3] = {64, (uint32_t)D, 1};
-    int32_t rc = make_map(&mv, vt, 3, dims, str, box);
+    int32_t rc = make_map(&mv, vt, 3, dims, str, box, dt);
     if (rc) return rc;
   }
   AttnTcParams p;
-  p.out = (bf16*)out; p.ldo = ldo; p.bso = L * ldo; p.L = (int)L; p.heads = (int)heads;
+  p.out = out; p.ldo = ldo; p.bso = L * ldo; p.L = (int)L; p.heads = (int)heads;
   p.scale_log2e = scale * 1.4426950408889634f;
-  return launch_self<2, 5, 80, 80>(mq, mk, mv, p, NB, (cudaStream_t)stream);
+  FYC_DISPATCH16(dt, return launch_self<2, 5, 80, 80, T>(mq, mk, mv, p, NB, (cudaStream_t)stream))
+  return FYC_OK;
 }
 
-// Cross-attention with a resident short context on tensor cores (head dim 40, 64 or 80).  q: [NB, Lq, ldq] bf16, head h at columns [q_col0 + D h, +D),
+// Cross-attention with a resident short context on tensor cores (head dim 40, 64 or 80).  q: [NB, Lq, ldq] 16-bit (dt), head h at columns [q_col0 + D h, +D),
 // UNPADDED, ldq >= heads * D;
 // k: [NBc, 80, ldk] with head h at columns [DKP h, +D), DKP = 64 for D = 40 (columns D..63 ZERO) or 64, 80 for D = 80, rows Lk..79 zero;
 // vt: [NBc, heads * D, 80]; optional second context k2 [NBc, 16, ldk2], vt2 [NBc, heads * D, 16] (rows / columns Lk2..15 zero).
 // out[n, i, h D + :] = out_alpha softmax_j<Lk(scale q k^T) v + alpha2 softmax_j<Lk2(scale q k2^T) v2, NBc = NB / kv_batch_div.
-extern "C" int32_t fyc_cross_attention_tc(const void* q, int64_t ldq, int64_t q_col0, const void* k, int64_t ldk, const void* vt,
+static int32_t cross_attention_tc(int32_t dt, const void* q, int64_t ldq, int64_t q_col0, const void* k, int64_t ldk, const void* vt,
                                           const void* k2, int64_t ldk2, const void* vt2, void* out, int64_t ldo, int64_t NB, int64_t heads,
                                           int64_t Lq, int64_t D, int64_t Lk, int64_t Lk2, int64_t kv_batch_div, float scale, float out_alpha,
                                           float alpha2, void* stream) {
@@ -488,19 +504,19 @@ extern "C" int32_t fyc_cross_attention_tc(const void* q, int64_t ldq, int64_t q_
     uint64_t dims[3] = {(uint64_t)(heads * D), (uint64_t)Lq, (uint64_t)NB};
     uint64_t str[2] = {(uint64_t)ldq * 2, (uint64_t)Lq * ldq * 2};
     uint32_t box[3] = {64, (uint32_t)BQ, 1};
-    int32_t rc = make_map(&mq, (const bf16*)q + q_col0, 3, dims, str, box);
+    int32_t rc = make_map(&mq, (const uint16_t*)q + q_col0, 3, dims, str, box, dt);
     if (rc) return rc;
   }
   {
     uint64_t dims[3] = {(uint64_t)(heads * DKP), (uint64_t)CX_LK, (uint64_t)NBc};
     uint64_t str[2] = {(uint64_t)ldk * 2, (uint64_t)CX_LK * ldk * 2};
     uint32_t box[3] = {64, (uint32_t)CX_LK, 1};
-    int32_t rc = make_map(&mk, k, 3, dims, str, box);
+    int32_t rc = make_map(&mk, k, 3, dims, str, box, dt);
     if (rc) return rc;
     uint64_t vd[3] = {(uint64_t)CX_LK, (uint64_t)(heads * D), (uint64_t)NBc};
     uint64_t vs[2] = {CX_LK * 2, (uint64_t)(CX_LK * heads * D * 2)};
     uint32_t vb[3] = {64, DV, 1};
-    rc = make_map(&mv, vt, 3, vd, vs, vb);
+    rc = make_map(&mv, vt, 3, vd, vs, vb, dt);
     if (rc) return rc;
   }
   mk2 = mk; mv2 = mv;
@@ -508,16 +524,16 @@ extern "C" int32_t fyc_cross_attention_tc(const void* q, int64_t ldq, int64_t q_
     uint64_t dims[3] = {(uint64_t)(heads * DKP), (uint64_t)CX_LK2, (uint64_t)NBc};
     uint64_t str[2] = {(uint64_t)ldk2 * 2, (uint64_t)CX_LK2 * ldk2 * 2};
     uint32_t box[3] = {64, (uint32_t)CX_LK2, 1};
-    int32_t rc = make_map(&mk2, k2, 3, dims, str, box);
+    int32_t rc = make_map(&mk2, k2, 3, dims, str, box, dt);
     if (rc) return rc;
     uint64_t vd[3] = {(uint64_t)CX_LK2, (uint64_t)(heads * D), (uint64_t)NBc};
     uint64_t vs[2] = {CX_LK2 * 2, (uint64_t)(CX_LK2 * heads * D * 2)};
     uint32_t vb[3] = {64, DV, 1};
-    rc = make_map(&mv2, vt2, 3, vd, vs, vb);
+    rc = make_map(&mv2, vt2, 3, vd, vs, vb, dt);
     if (rc) return rc;
   }
   AttnCxParams p;
-  p.out = (bf16*)out; p.ldo = ldo; p.bso = Lq * ldo; p.Lq = (int)Lq; p.heads = (int)heads; p.Lk = (int)Lk; p.Lk2 = (int)Lk2;
+  p.out = out; p.ldo = ldo; p.bso = Lq * ldo; p.Lq = (int)Lq; p.heads = (int)heads; p.Lk = (int)Lk; p.Lk2 = (int)Lk2;
   p.kv_div = (int)kv_batch_div; p.scale_log2e = scale * 1.4426950408889634f; p.out_alpha = out_alpha; p.alpha2 = alpha2;
   p.nqt = (int)((Lq + BQ - 1) / BQ);
   // CTAs per (image, head): enough to fill the machine once (one CTA per SM), at most one per pair of query tiles - the context load is
@@ -527,25 +543,41 @@ extern "C" int32_t fyc_cross_attention_tc(const void* q, int64_t ldq, int64_t q_
   if (gx > (p.nqt + 1) / 2) gx = (p.nqt + 1) / 2;
   dim3 grid((unsigned)gx, (unsigned)heads, (unsigned)NB);
   cudaStream_t st = (cudaStream_t)stream;
-  if (D == 40) {
-    constexpr int smem = cx_smem<1, 48>();
-    auto kern = attention_cx_kernel<1, 3, 48, 40>;
-    static bool attr = false;
-    if (!attr) { FYC_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem)); attr = true; }
-    kern<<<grid, NTHREADS, smem, st>>>(mq, mk, mv, mk2, mv2, p);
-  } else if (D == 64) {
-    constexpr int smem = cx_smem<1, 64>();
-    auto kern = attention_cx_kernel<1, 4, 64, 64>;
-    static bool attr = false;
-    if (!attr) { FYC_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem)); attr = true; }
-    kern<<<grid, NTHREADS, smem, st>>>(mq, mk, mv, mk2, mv2, p);
-  } else {
-    constexpr int smem = cx_smem<2, 80>();
-    auto kern = attention_cx_kernel<2, 5, 80, 80>;
-    static bool attr = false;
-    if (!attr) { FYC_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem)); attr = true; }
-    kern<<<grid, NTHREADS, smem, st>>>(mq, mk, mv, mk2, mv2, p);
-  }
-  FYC_LAUNCH_CHECK();
+  FYC_DISPATCH16(dt, {
+    if (D == 40) return launch_cx<1, 3, 48, 40, T>(mq, mk, mv, mk2, mv2, p, grid, st);
+    if (D == 64) return launch_cx<1, 4, 64, 64, T>(mq, mk, mv, mk2, mv2, p, grid, st);
+    return launch_cx<2, 5, 80, 80, T>(mq, mk, mv, mk2, mv2, p, grid, st);
+  })
   return FYC_OK;
+}
+
+extern "C" int32_t fyc_self_attention_tc(const void* qk, int64_t ldqk, int64_t q_col0, int64_t k_col0, const void* vt, void* out,
+                                         int64_t ldo, int64_t NB, int64_t heads, int64_t L, int64_t D, float scale, void* stream) {
+  return self_attention_tc(FYC_BF16, qk, ldqk, q_col0, k_col0, vt, out, ldo, NB, heads, L, D, scale, stream);
+}
+extern "C" int32_t fyc_self_attention_tc_f16(const void* qk, int64_t ldqk, int64_t q_col0, int64_t k_col0, const void* vt, void* out,
+                                             int64_t ldo, int64_t NB, int64_t heads, int64_t L, int64_t D, float scale, void* stream) {
+  return self_attention_tc(FYC_F16, qk, ldqk, q_col0, k_col0, vt, out, ldo, NB, heads, L, D, scale, stream);
+}
+extern "C" int32_t fyc_self_attention_tc_d80(const void* qkv, int64_t ldqkv, int64_t q_col0, int64_t k_col0, const void* vt, void* out,
+                                             int64_t ldo, int64_t NB, int64_t heads, int64_t L, float scale, void* stream) {
+  return self_attention_tc_d80(FYC_BF16, qkv, ldqkv, q_col0, k_col0, vt, out, ldo, NB, heads, L, scale, stream);
+}
+extern "C" int32_t fyc_self_attention_tc_d80_f16(const void* qkv, int64_t ldqkv, int64_t q_col0, int64_t k_col0, const void* vt, void* out,
+                                                 int64_t ldo, int64_t NB, int64_t heads, int64_t L, float scale, void* stream) {
+  return self_attention_tc_d80(FYC_F16, qkv, ldqkv, q_col0, k_col0, vt, out, ldo, NB, heads, L, scale, stream);
+}
+extern "C" int32_t fyc_cross_attention_tc(const void* q, int64_t ldq, int64_t q_col0, const void* k, int64_t ldk, const void* vt,
+                                          const void* k2, int64_t ldk2, const void* vt2, void* out, int64_t ldo, int64_t NB, int64_t heads,
+                                          int64_t Lq, int64_t D, int64_t Lk, int64_t Lk2, int64_t kv_batch_div, float scale, float out_alpha,
+                                          float alpha2, void* stream) {
+  return cross_attention_tc(FYC_BF16, q, ldq, q_col0, k, ldk, vt, k2, ldk2, vt2, out, ldo, NB, heads, Lq, D, Lk, Lk2, kv_batch_div, scale,
+                            out_alpha, alpha2, stream);
+}
+extern "C" int32_t fyc_cross_attention_tc_f16(const void* q, int64_t ldq, int64_t q_col0, const void* k, int64_t ldk, const void* vt,
+                                              const void* k2, int64_t ldk2, const void* vt2, void* out, int64_t ldo, int64_t NB, int64_t heads,
+                                              int64_t Lq, int64_t D, int64_t Lk, int64_t Lk2, int64_t kv_batch_div, float scale, float out_alpha,
+                                              float alpha2, void* stream) {
+  return cross_attention_tc(FYC_F16, q, ldq, q_col0, k, ldk, vt, k2, ldk2, vt2, out, ldo, NB, heads, Lq, D, Lk, Lk2, kv_batch_div, scale,
+                            out_alpha, alpha2, stream);
 }

@@ -1,12 +1,16 @@
 // Shared helpers for libfyc_sm90a (H100 / sm_90a only).
 #pragma once
 #include <cuda_bf16.h>
+#include <cuda_fp16.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
+
+#include <type_traits>
 
 #include "fyc.h"
 
 typedef __nv_bfloat16 bf16;
+typedef __half f16;
 
 void fyc_set_error(const char* fmt, ...);
 
@@ -34,29 +38,60 @@ void fyc_set_error(const char* fmt, ...);
   switch (dt) {                                                \
     case FYC_F32: { using T = float; __VA_ARGS__; } break;     \
     case FYC_BF16: { using T = bf16; __VA_ARGS__; } break;     \
+    case FYC_F16: { using T = f16; __VA_ARGS__; } break;       \
     default: FYC_CHECK(false, "unknown dtype %d", (int)(dt));  \
   }
+// the same over the 16-bit storage dtypes only (the tensor-core paths)
+#define FYC_DISPATCH16(dt, ...)                                       \
+  switch (dt) {                                                       \
+    case FYC_BF16: { using T = bf16; __VA_ARGS__; } break;            \
+    case FYC_F16: { using T = f16; __VA_ARGS__; } break;              \
+    default: FYC_CHECK(false, "unsupported 16-bit dtype %d", (int)(dt)); \
+  }
+static inline bool fyc_is_16bit(int32_t dt) { return dt == FYC_BF16 || dt == FYC_F16; }
 
 __device__ __forceinline__ float to_f(float v) { return v; }
 __device__ __forceinline__ float to_f(bf16 v) { return __bfloat162float(v); }
 template <typename T> __device__ __forceinline__ T from_f(float v);
 template <> __device__ __forceinline__ float from_f<float>(float v) { return v; }
 template <> __device__ __forceinline__ bf16 from_f<bf16>(float v) { return __float2bfloat16_rn(v); }
+__device__ __forceinline__ float to_f(f16 v) { return __half2float(v); }
+template <> __device__ __forceinline__ f16 from_f<f16>(float v) { return __float2half_rn(v); }
 
-// 8-element vector of T (16 B for bf16, 32 B for fp32) <-> float[8]
-template <typename T> struct Vec8;
-template <> struct Vec8<bf16> {
-  static __device__ __forceinline__ void load(const bf16* p, float* f) {
+// Two 16-bit values in one 32-bit word (element 0 in the low half): Pair16<T>::type is __nv_bfloat162 | __half2, pack() rounds two
+// floats once, unpack() widens exactly; ONE is the bit pattern of 1.0.
+template <typename T> struct Pair16;
+template <> struct Pair16<bf16> {
+  typedef __nv_bfloat162 type;
+  static constexpr uint32_t ONE = 0x3F80u;
+  static __device__ __forceinline__ type pack(float lo, float hi) { return __floats2bfloat162_rn(lo, hi); }
+  static __device__ __forceinline__ float2 unpack(type v) { return __bfloat1622float2(v); }
+};
+template <> struct Pair16<f16> {
+  typedef __half2 type;
+  static constexpr uint32_t ONE = 0x3C00u;
+  static __device__ __forceinline__ type pack(float lo, float hi) { return __floats2half2_rn(lo, hi); }
+  static __device__ __forceinline__ float2 unpack(type v) { return __half22float2(v); }
+};
+template <typename T> __device__ __forceinline__ uint32_t pack_u32(float lo, float hi) {
+  typename Pair16<T>::type v = Pair16<T>::pack(lo, hi);
+  return *reinterpret_cast<uint32_t*>(&v);
+}
+
+// 8-element vector of T (16 B for bf16 / fp16, 32 B for fp32) <-> float[8]
+template <typename T> struct Vec8 {     // 16-bit T
+  typedef typename Pair16<T>::type P;
+  static __device__ __forceinline__ void load(const T* p, float* f) {
     uint4 u = *reinterpret_cast<const uint4*>(p);
-    const __nv_bfloat162* h = reinterpret_cast<const __nv_bfloat162*>(&u);
+    const P* h = reinterpret_cast<const P*>(&u);
 #pragma unroll
-    for (int i = 0; i < 4; ++i) { float2 t = __bfloat1622float2(h[i]); f[2 * i] = t.x; f[2 * i + 1] = t.y; }
+    for (int i = 0; i < 4; ++i) { float2 t = Pair16<T>::unpack(h[i]); f[2 * i] = t.x; f[2 * i + 1] = t.y; }
   }
-  static __device__ __forceinline__ void store(bf16* p, const float* f) {
+  static __device__ __forceinline__ void store(T* p, const float* f) {
     uint4 u;
-    __nv_bfloat162* h = reinterpret_cast<__nv_bfloat162*>(&u);
+    P* h = reinterpret_cast<P*>(&u);
 #pragma unroll
-    for (int i = 0; i < 4; ++i) h[i] = __floats2bfloat162_rn(f[2 * i], f[2 * i + 1]);
+    for (int i = 0; i < 4; ++i) h[i] = Pair16<T>::pack(f[2 * i], f[2 * i + 1]);
     *reinterpret_cast<uint4*>(p) = u;
   }
 };
@@ -72,19 +107,19 @@ template <> struct Vec8<float> {
 };
 
 // 4-element vector
-template <typename T> struct Vec4;
-template <> struct Vec4<bf16> {
-  static __device__ __forceinline__ void load(const bf16* p, float* f) {
+template <typename T> struct Vec4 {     // 16-bit T
+  typedef typename Pair16<T>::type P;
+  static __device__ __forceinline__ void load(const T* p, float* f) {
     uint2 u = *reinterpret_cast<const uint2*>(p);
-    const __nv_bfloat162* h = reinterpret_cast<const __nv_bfloat162*>(&u);
-    float2 a = __bfloat1622float2(h[0]), b = __bfloat1622float2(h[1]);
+    const P* h = reinterpret_cast<const P*>(&u);
+    float2 a = Pair16<T>::unpack(h[0]), b = Pair16<T>::unpack(h[1]);
     f[0] = a.x; f[1] = a.y; f[2] = b.x; f[3] = b.y;
   }
-  static __device__ __forceinline__ void store(bf16* p, const float* f) {
+  static __device__ __forceinline__ void store(T* p, const float* f) {
     uint2 u;
-    __nv_bfloat162* h = reinterpret_cast<__nv_bfloat162*>(&u);
-    h[0] = __floats2bfloat162_rn(f[0], f[1]);
-    h[1] = __floats2bfloat162_rn(f[2], f[3]);
+    P* h = reinterpret_cast<P*>(&u);
+    h[0] = Pair16<T>::pack(f[0], f[1]);
+    h[1] = Pair16<T>::pack(f[2], f[3]);
     *reinterpret_cast<uint2*>(p) = u;
   }
 };
@@ -110,8 +145,19 @@ template <typename T, int V> __device__ __forceinline__ void store_vec(T* p, con
   else *p = from_f<T>(f[0]);
 }
 
+// mma.sync m16n8k16, fp32 accumulator c += a b with 16-bit operands T (bf16 | f16)
+template <typename T> __device__ __forceinline__ void mma16816(float* c, const uint32_t* a, uint32_t b0, uint32_t b1) {
+  if constexpr (std::is_same<T, f16>::value)
+    asm volatile("mma.sync.aligned.m16n8k16.row.col.f32.f16.f16.f32 {%0, %1, %2, %3}, {%4, %5, %6, %7}, {%8, %9}, {%0, %1, %2, %3};"
+                 : "+f"(c[0]), "+f"(c[1]), "+f"(c[2]), "+f"(c[3])
+                 : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
+  else
+    asm volatile("mma.sync.aligned.m16n8k16.row.col.f32.bf16.bf16.f32 {%0, %1, %2, %3}, {%4, %5, %6, %7}, {%8, %9}, {%0, %1, %2, %3};"
+                 : "+f"(c[0]), "+f"(c[1]), "+f"(c[2]), "+f"(c[3])
+                 : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
+}
 __device__ __forceinline__ float silu_f(float x) { return x / (1.0f + expf(-x)); }
-// bf16-storage paths: 2-ulp intrinsics are far below the 2^-9 output rounding
+// 16-bit-storage paths: 2-ulp intrinsics are far below the 2^-9 (bf16) / 2^-12 (fp16) output rounding
 __device__ __forceinline__ float silu_fast(float x) { return __fdividef(x, 1.0f + __expf(-x)); }
 // exact-erf GELU (F.gelu default; diffusers/models/attention.py:815)
 __device__ __forceinline__ float gelu_erf_f(float x) { return 0.5f * x * (1.0f + erff(x * 0.70710678118654752440f)); }

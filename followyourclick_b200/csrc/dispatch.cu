@@ -27,7 +27,7 @@ extern "C" int32_t fyc_gemm(const fyc_gemm_args* g, void* stream) {
   FYC_CHECK(!(g->epilogue & FYC_EPI_BIAS) || g->bias, "gemm: FYC_EPI_BIAS without bias");
   FYC_CHECK(!(g->epilogue & FYC_EPI_RESIDUAL) || g->residual, "gemm: FYC_EPI_RESIDUAL without residual");
   FYC_CHECK(!(g->epilogue & FYC_EPI_ROWBIAS) || (g->rowbias && g->rows_per_group > 0), "gemm: FYC_EPI_ROWBIAS without rowbias/rows_per_group");
-  FYC_CHECK(!(g->epilogue & FYC_EPI_OUT_F32) || g->dtype == FYC_BF16 || g->dtype == FYC_F32, "gemm: bad dtype");
+  FYC_CHECK(!(g->epilogue & FYC_EPI_OUT_F32) || fyc_is_16bit(g->dtype) || g->dtype == FYC_F32, "gemm: bad dtype");
   if (g->A2)
     FYC_CHECK(g->impl != FYC_IMPL_SIMT && fyc_gemm_tc_eligible(g), "gemm: the two-segment A (A2) is a tensor-core-path feature (bf16, K1 %% 64 == 0); "
               "other callers materialise the concatenation with fyc_concat_channels");
@@ -41,7 +41,7 @@ extern "C" int32_t fyc_gemm(const fyc_gemm_args* g, void* stream) {
 }
 
 extern "C" size_t fyc_conv3x3_workspace_bytes(const fyc_conv3x3_args* c) {
-  if (c->dtype == FYC_BF16 && c->stride == 2 && c->upsample == 1) return (size_t)(c->NB * c->H * c->W * c->Cin * 2);
+  if (fyc_is_16bit(c->dtype) && c->stride == 2 && c->upsample == 1) return (size_t)(c->NB * c->H * c->W * c->Cin * 2);
   return 0;
 }
 

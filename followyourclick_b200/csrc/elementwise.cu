@@ -99,7 +99,7 @@ __global__ void upsample2x_kernel(const T* __restrict__ x, T* __restrict__ out, 
 extern "C" int32_t fyc_upsample_nearest2x(const void* x, void* out, int64_t NB, int64_t H, int64_t W, int64_t C,
                                           int32_t dtype, void* stream) {
   cudaStream_t st = (cudaStream_t)stream;
-  if (dtype == FYC_BF16 && C % 8 == 0) {
+  if (fyc_is_16bit(dtype) && C % 8 == 0) {     // a 16-byte copy: the bf16 instantiation moves any 16-bit type
     upsample2x_kernel<bf16, 8><<<grid_for(NB * 4 * H * W * C / 8, 256), 256, 0, st>>>((const bf16*)x, (bf16*)out, NB, H, W, C);
   } else {
     FYC_DISPATCH(dtype, upsample2x_kernel<T, 1><<<grid_for(NB * 4 * H * W * C, 256), 256, 0, st>>>((const T*)x, (T*)out, NB, H, W, C));
@@ -124,7 +124,7 @@ __global__ void concat_kernel(const T* __restrict__ a, const T* __restrict__ b, 
 extern "C" int32_t fyc_concat_channels(const void* a, const void* b, void* out, int64_t M, int64_t C1, int64_t C2,
                                        int32_t dtype, void* stream) {
   cudaStream_t st = (cudaStream_t)stream;
-  if (dtype == FYC_BF16 && C1 % 8 == 0 && C2 % 8 == 0) {
+  if (fyc_is_16bit(dtype) && C1 % 8 == 0 && C2 % 8 == 0) {     // a 16-byte copy: the bf16 instantiation moves any 16-bit type
     concat_kernel<bf16, 8><<<grid_for(M * (C1 + C2) / 8, 256), 256, 0, st>>>((const bf16*)a, (const bf16*)b, (bf16*)out, M, C1, C2);
   } else if (dtype == FYC_F32 && C1 % 4 == 0 && C2 % 4 == 0) {
     concat_kernel<float, 4><<<grid_for(M * (C1 + C2) / 4, 256), 256, 0, st>>>((const float*)a, (const float*)b, (float*)out, M, C1, C2);
@@ -278,7 +278,12 @@ __global__ void frames_finalize_kernel(const T* __restrict__ x, float* __restric
     int64_t c = r % 3; int64_t bi = r / 3;
     float v = to_f(x[((bi * F + f) * HW + p) * ldc + c]);
     v = __fadd_rn(__fdiv_rn(v, 2.0f), 0.5f);
-    video[i] = fminf(fmaxf(v, 0.f), 1.f);
+    if constexpr (std::is_same<T, f16>::value)
+      // fp16 storage ends at 65504: a value that overflowed anywhere upstream (inf, or the NaN it turns into) reaches the video as NaN
+      // instead of being clipped to a black or white pixel (fminf / fmaxf return the non-NaN operand)
+      video[i] = isfinite(v) ? fminf(fmaxf(v, 0.f), 1.f) : __int_as_float(0x7fffffff);
+    else
+      video[i] = fminf(fmaxf(v, 0.f), 1.f);
   }
 }
 extern "C" int32_t fyc_frames_finalize(const void* x, float* video, int64_t b, int64_t F, int64_t HW, int64_t ldc, int32_t dtype, void* stream) {

@@ -2,7 +2,7 @@
 //
 // Role: (1) the strict-fp32 parity path (dtype = FYC_F32: every product and sum in fp32, the on-GPU
 // restatement the tensor-core kernels are themselves checked against), and (2) shapes the tensor-core path does not
-// take (Cin = 9 / 4 stems, Cout = 4 / 3 heads, M = 2 time-embedding MLPs).  The bf16 hot path is gemm_tc.cu.
+// take (Cin = 9 / 4 stems, Cout = 4 / 3 heads, M = 2 time-embedding MLPs).  The 16-bit hot path is gemm_tc.cu.
 //
 // Tiling: 128 x 64 x 16 CTA tile, 256 threads, 8 x 4 register tile per thread, smem double buffering with
 // register prefetch.  The A-operand loader is a functor so the same main loop serves plain row-major A and the
@@ -185,11 +185,13 @@ int32_t fyc_gemm_simt(const fyc_gemm_args* g, cudaStream_t st) {
     PlainAS<float> al; al.A = (const float*)g->A; al.lda = g->lda; al.M = g->M; al.K = g->K;
     al.vec = (g->K % 8 == 0) && (g->lda % 8 == 0) && (((uintptr_t)g->A) % 32 == 0) && (g->strideA % 8 == 0);
     return launch<float, float>(al, (const float*)g->W, (float*)g->out, g->M, g->N, g->K, g->ldw, g->batch, g->strideA, g->strideW, g->strideO, ep, st);
-  } else if (g->dtype == FYC_BF16) {
-    PlainAS<bf16> al; al.A = (const bf16*)g->A; al.lda = g->lda; al.M = g->M; al.K = g->K;
-    al.vec = (g->K % 8 == 0) && (g->lda % 8 == 0) && (((uintptr_t)g->A) % 16 == 0) && (g->strideA % 8 == 0);
-    if (f32out) return launch<bf16, float>(al, (const bf16*)g->W, (float*)g->out, g->M, g->N, g->K, g->ldw, g->batch, g->strideA, g->strideW, g->strideO, ep, st);
-    return launch<bf16, bf16>(al, (const bf16*)g->W, (bf16*)g->out, g->M, g->N, g->K, g->ldw, g->batch, g->strideA, g->strideW, g->strideO, ep, st);
+  } else if (fyc_is_16bit(g->dtype)) {
+    FYC_DISPATCH16(g->dtype, {
+      PlainAS<T> al; al.A = (const T*)g->A; al.lda = g->lda; al.M = g->M; al.K = g->K;
+      al.vec = (g->K % 8 == 0) && (g->lda % 8 == 0) && (((uintptr_t)g->A) % 16 == 0) && (g->strideA % 8 == 0);
+      if (f32out) return launch<T, float>(al, (const T*)g->W, (float*)g->out, g->M, g->N, g->K, g->ldw, g->batch, g->strideA, g->strideW, g->strideO, ep, st);
+      return launch<T, T>(al, (const T*)g->W, (T*)g->out, g->M, g->N, g->K, g->ldw, g->batch, g->strideA, g->strideW, g->strideO, ep, st);
+    })
   }
   FYC_CHECK(false, "gemm: unknown dtype %d", g->dtype);
 }
@@ -206,11 +208,13 @@ int32_t fyc_conv3x3_simt(const fyc_conv3x3_args* c, cudaStream_t st) {
     ConvAS<float> al; al.x = (const float*)c->x; al.NB = c->NB; al.H = c->H; al.W = c->W; al.Cin = c->Cin; al.Ho = Ho; al.Wo = Wo;
     al.M = M; al.K = K; al.stride = s; al.up = up; al.pad = pad; al.vec = (c->Cin % 8 == 0) && (((uintptr_t)c->x) % 32 == 0);
     return launch<float, float>(al, (const float*)c->w, (float*)c->out, M, N, K, K, 1, 0, 0, 0, ep, st);
-  } else if (c->dtype == FYC_BF16) {
-    ConvAS<bf16> al; al.x = (const bf16*)c->x; al.NB = c->NB; al.H = c->H; al.W = c->W; al.Cin = c->Cin; al.Ho = Ho; al.Wo = Wo;
-    al.M = M; al.K = K; al.stride = s; al.up = up; al.pad = pad; al.vec = (c->Cin % 8 == 0) && (((uintptr_t)c->x) % 16 == 0);
-    if (f32out) return launch<bf16, float>(al, (const bf16*)c->w, (float*)c->out, M, N, K, K, 1, 0, 0, 0, ep, st);
-    return launch<bf16, bf16>(al, (const bf16*)c->w, (bf16*)c->out, M, N, K, K, 1, 0, 0, 0, ep, st);
+  } else if (fyc_is_16bit(c->dtype)) {
+    FYC_DISPATCH16(c->dtype, {
+      ConvAS<T> al; al.x = (const T*)c->x; al.NB = c->NB; al.H = c->H; al.W = c->W; al.Cin = c->Cin; al.Ho = Ho; al.Wo = Wo;
+      al.M = M; al.K = K; al.stride = s; al.up = up; al.pad = pad; al.vec = (c->Cin % 8 == 0) && (((uintptr_t)c->x) % 16 == 0);
+      if (f32out) return launch<T, float>(al, (const T*)c->w, (float*)c->out, M, N, K, K, 1, 0, 0, 0, ep, st);
+      return launch<T, T>(al, (const T*)c->w, (T*)c->out, M, N, K, K, 1, 0, 0, 0, ep, st);
+    })
   }
   FYC_CHECK(false, "conv3x3: unknown dtype %d", c->dtype);
 }

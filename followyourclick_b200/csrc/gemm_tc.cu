@@ -5,7 +5,7 @@
 // One persistent CTA per SM, 9 warps:
 //   warp 8 (1 lane)  TMA producer : cp.async.bulk.tensor (4-D box for the activation patch, 3-D box for the weight slab) into a
 //                                   3- or 4-stage 128B-swizzled shared-memory ring, mbarrier expect_tx
-//   warps 0..7       two consumer warpgroups, 64 rows of the 128-row tile each: wgmma.mma_async m64 x BN x 16 (bf16 -> fp32
+//   warps 0..7       two consumer warpgroups, 64 rows of the 128-row tile each: wgmma.mma_async m64 x BN x 16 (bf16 or fp16 -> fp32
 //                    register accumulators) straight from the swizzled stages, then the fused epilogue (bias / time-embedding
 //                    row bias / residual / GEGLU / LayerNorm fold / alpha) on the registers into the warpgroup's own shared-memory
 //                    staging buffer, which one thread writes out with TMA stores (clipped at the output's true extent).
@@ -154,7 +154,7 @@ __device__ __forceinline__ uint32_t stage_off(int row, int col, int esize) {
 // The accumulator of warpgroup wg holds rows wg*64 + 16*warp + lane/4 (+8) of the tile; n-tile j (8 columns) sits in acc[4j .. 4j+3]:
 // columns 8j + 2(lane%4) + {0, 1} of the first row, then of the second.  The results go to the warpgroup's staging buffer `stg`,
 // which holds the residual half-tile on entry when there is one; each thread reads its residual where it then writes its result.
-template <int BN>
+template <int BN, typename T>
 __device__ __forceinline__ void epilogue(const TcParams& p, const TileCoord& c, const float* acc, int wg, int warp4, int lane, uint8_t* stg) {
   const int q = lane & 3;
   const int flags = p.flags;
@@ -180,7 +180,7 @@ __device__ __forceinline__ void epilogue(const TcParams& p, const TileCoord& c, 
           const float g0 = acc[4 * (j + 16) + 2 * half], g1 = acc[4 * (j + 16) + 2 * half + 1];
           const float x = fmaf(a0, rs, ba.x) * gelu_erf_fast(fmaf(g0, rs, bg.x));
           const float y = fmaf(a1, rs, ba.y) * gelu_erf_fast(fmaf(g1, rs, bg.y));
-          *reinterpret_cast<__nv_bfloat162*>(stg + stage_off(row, col, 2)) = __floats2bfloat162_rn(x, y);
+          *reinterpret_cast<typename Pair16<T>::type*>(stg + stage_off(row, col, 2)) = Pair16<T>::pack(x, y);
         }
       }
       continue;
@@ -198,16 +198,17 @@ __device__ __forceinline__ void epilogue(const TcParams& p, const TileCoord& c, 
         if (has_res) { const float2 r = *s; x += r.x; y += r.y; }
         *s = make_float2(x, y);
       } else {
-        __nv_bfloat162* s = reinterpret_cast<__nv_bfloat162*>(stg + stage_off(row, col, 2));
-        if (has_res) { const float2 r = __bfloat1622float2(*s); x += r.x; y += r.y; }
-        *s = __floats2bfloat162_rn(x, y);
+        typename Pair16<T>::type* s = reinterpret_cast<typename Pair16<T>::type*>(stg + stage_off(row, col, 2));
+        if (has_res) { const float2 r = Pair16<T>::unpack(*s); x += r.x; y += r.y; }
+        *s = Pair16<T>::pack(x, y);
       }
     }
   }
 }
 
 // ---------------------------------------------------------------------------------------------- kernel
-template <int BN>
+// T: the 16-bit operand / output type (bf16 | f16)
+template <int BN, typename T>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
 gemm_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_w, const __grid_constant__ CUtensorMap map_a2,
                const __grid_constant__ CUtensorMap map_out, const __grid_constant__ CUtensorMap map_res, const TcParams p) {
@@ -315,7 +316,7 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
       wgmma_fence();
 #pragma unroll
       for (int kk = 0; kk < BK / 16; ++kk)
-        Wgmma<BN>::ss(acc, a_desc + (uint64_t)(2 * kk), b_desc + (uint64_t)(2 * kk), (k > 0 || kk > 0) ? 1 : 0);
+        Wgmma<BN, T>::ss(acc, a_desc + (uint64_t)(2 * kk), b_desc + (uint64_t)(2 * kk), (k > 0 || kk > 0) ? 1 : 0);
       wgmma_commit();
       wgmma_wait<1>();                                   // the previous stage's MMAs have retired: hand it back to the producer
       if (prev >= 0) mbar_arrive(&empty[prev]);
@@ -330,7 +331,7 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
     if (elected) bulk_wait_read();
     warpgroup_sync(wg);                                          // the staging buffer is free (and holds the residual, if any)
     if (has_res) { mbar_wait(&rbar[wg], rphase); rphase ^= 1; }
-    epilogue<BN>(p, tile_coord(p, tile), acc, wg, warp4, lane, stg());
+    epilogue<BN, T>(p, tile_coord(p, tile), acc, wg, warp4, lane, stg());
     fence_async_smem();
     warpgroup_sync(wg);
     if (elected) {
@@ -342,7 +343,8 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
   if (elected) bulk_wait_all();
 }
 
-// parity-plane split for stride-2 convolutions: x [NB, H, W, C] -> planes [4, NB, H/2, W/2, C], plane = 2*(h&1) + (w&1)
+// parity-plane split for stride-2 convolutions: x [NB, H, W, C] -> planes [4, NB, H/2, W/2, C], plane = 2*(h&1) + (w&1).  A pure copy of
+// 16-byte vectors: it serves every 16-bit element type.
 __global__ void space_to_planes_kernel(const bf16* __restrict__ x, bf16* __restrict__ out, int64_t NB, int64_t H, int64_t W, int64_t C) {
   const int64_t cv = C / 8, H2 = H / 2, W2 = W / 2;
   const int64_t total = NB * H * W * cv;
@@ -377,9 +379,11 @@ EncodeTiledFn get_encode_fn() {
   return fn;
 }
 
+// TMA element type of a 16-bit storage dtype (FYC_BF16 | FYC_F16)
+CUtensorMapDataType map_dtype(int32_t dt) { return dt == FYC_F16 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16; }
+
 int32_t encode_map(CUtensorMap* m, const void* base, int rank, const uint64_t* dims, const uint64_t* strides_bytes,
-                   const uint32_t* box, CUtensorMapDataType dtype = CU_TENSOR_MAP_DATA_TYPE_BFLOAT16,
-                   CUtensorMapSwizzle swizzle = CU_TENSOR_MAP_SWIZZLE_128B) {
+                   const uint32_t* box, CUtensorMapDataType dtype, CUtensorMapSwizzle swizzle = CU_TENSOR_MAP_SWIZZLE_128B) {
   EncodeTiledFn fn = get_encode_fn();
   FYC_CHECK(fn != nullptr, "tensor-core path: cuTensorMapEncodeTiled driver entry point unavailable");
   cuuint64_t gdim[5]; cuuint64_t gstr[4]; cuuint32_t bx[5]; cuuint32_t es[5];
@@ -397,7 +401,7 @@ int32_t encode_map(CUtensorMap* m, const void* base, int rank, const uint64_t* d
 // Output (or residual) map of a launch: `cols` channels by W x H x NB pixels at `base`, pixel (w, h, n) at element offset
 // w * sw + h * sh + n * sn.  The dimensions are the tensor's true extent, so TMA clips the rows past M and the columns past N_out.
 // Box: one 32-byte column box of a warpgroup's half patch (choose_tiles sets the split).
-int32_t encode_out_map(CUtensorMap* m, const void* base, const TcParams& p, uint64_t cols, uint64_t W, uint64_t H, uint64_t NB,
+int32_t encode_out_map(CUtensorMap* m, const void* base, const TcParams& p, int32_t dt, uint64_t cols, uint64_t W, uint64_t H, uint64_t NB,
                        uint64_t sw, uint64_t sh, uint64_t sn) {
   const bool f32 = (p.flags & FYC_EPI_OUT_F32) != 0;
   const uint64_t es = f32 ? 4 : 2;
@@ -405,7 +409,7 @@ int32_t encode_out_map(CUtensorMap* m, const void* base, const TcParams& p, uint
   uint64_t str[3] = {sw * es, sh * es, sn * es};
   uint32_t box[4] = {(uint32_t)(OUT_BOX_BYTES / es), (uint32_t)(p.half_dw ? p.half_dw : p.bw), (uint32_t)(p.half_dh ? p.half_dh : p.bh),
                      (uint32_t)(p.half_dn ? p.half_dn : p.bn)};
-  return encode_map(m, base, 4, dims, str, box, f32 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16,
+  return encode_map(m, base, 4, dims, str, box, f32 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : map_dtype(dt),
                     CU_TENSOR_MAP_SWIZZLE_32B);
 }
 
@@ -501,23 +505,23 @@ void choose_tiles(TcParams& p, int* grid_out) {
   *grid_out = grid;
 }
 
-template <int BN>
+template <int BN, typename T>
 int32_t launch_bn(const CUtensorMap& ma, const CUtensorMap& mw, const CUtensorMap& ma2, const CUtensorMap& mo, const CUtensorMap& mr,
                   const TcParams& p, int grid, cudaStream_t st) {
   static bool attr_set = false;
   if (!attr_set) {
-    FYC_CUDA(cudaFuncSetAttribute(gemm_tc_kernel<BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_LIMIT));
+    FYC_CUDA(cudaFuncSetAttribute(gemm_tc_kernel<BN, T>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_LIMIT));
     attr_set = true;
   }
   const int smem = p.ring_bytes + 2 * p.stg_bytes + SMEM_EXTRA;
   FYC_CHECK(smem <= SMEM_LIMIT && p.a_stages >= 2 && p.a_stages <= MAX_STAGES, "tensor-core GEMM: shared-memory plan does not fit (BN %d)", BN);
-  gemm_tc_kernel<BN><<<grid, NUM_THREADS, smem, st>>>(ma, mw, ma2, mo, mr, p);
+  gemm_tc_kernel<BN, T><<<grid, NUM_THREADS, smem, st>>>(ma, mw, ma2, mo, mr, p);
   FYC_LAUNCH_CHECK();
   return FYC_OK;
 }
 
 // mr: the residual map (FYC_EPI_RESIDUAL only; otherwise unused)
-int32_t launch_tc(const CUtensorMap& ma, const CUtensorMap& mw, const CUtensorMap& mo, const CUtensorMap* mr, TcParams p, int grid,
+int32_t launch_tc(int32_t dt, const CUtensorMap& ma, const CUtensorMap& mw, const CUtensorMap& mo, const CUtensorMap* mr, TcParams p, int grid,
                   cudaStream_t st, const CUtensorMap* ma2p = nullptr) {
   const CUtensorMap& ma2 = ma2p ? *ma2p : ma;
   const CUtensorMap& mres = mr ? *mr : mo;
@@ -529,18 +533,18 @@ int32_t launch_tc(const CUtensorMap& ma, const CUtensorMap& mw, const CUtensorMa
   const int64_t tiles = p.m_tiles * p.n_tiles;
   FYC_CHECK(tiles < (1ll << 31) && p.M < (1ll << 31) && p.rows_per_group < (1ll << 31), "tensor-core GEMM: problem exceeds the 32-bit tile index range");
   if (grid > tiles) grid = (int)tiles;
-  switch (p.BN) {
-    case 256: return launch_bn<256>(ma, mw, ma2, mo, mres, p, grid, st);
-    case 192: return launch_bn<192>(ma, mw, ma2, mo, mres, p, grid, st);
-    case 160: return launch_bn<160>(ma, mw, ma2, mo, mres, p, grid, st);
-    case 128: return launch_bn<128>(ma, mw, ma2, mo, mres, p, grid, st);
-    case 96: return launch_bn<96>(ma, mw, ma2, mo, mres, p, grid, st);
-    case 80: return launch_bn<80>(ma, mw, ma2, mo, mres, p, grid, st);
-    case 64: return launch_bn<64>(ma, mw, ma2, mo, mres, p, grid, st);
-    case 48: return launch_bn<48>(ma, mw, ma2, mo, mres, p, grid, st);
-    case 32: return launch_bn<32>(ma, mw, ma2, mo, mres, p, grid, st);
-    case 16: return launch_bn<16>(ma, mw, ma2, mo, mres, p, grid, st);
-  }
+  FYC_DISPATCH16(dt, switch (p.BN) {
+    case 256: return launch_bn<256, T>(ma, mw, ma2, mo, mres, p, grid, st);
+    case 192: return launch_bn<192, T>(ma, mw, ma2, mo, mres, p, grid, st);
+    case 160: return launch_bn<160, T>(ma, mw, ma2, mo, mres, p, grid, st);
+    case 128: return launch_bn<128, T>(ma, mw, ma2, mo, mres, p, grid, st);
+    case 96: return launch_bn<96, T>(ma, mw, ma2, mo, mres, p, grid, st);
+    case 80: return launch_bn<80, T>(ma, mw, ma2, mo, mres, p, grid, st);
+    case 64: return launch_bn<64, T>(ma, mw, ma2, mo, mres, p, grid, st);
+    case 48: return launch_bn<48, T>(ma, mw, ma2, mo, mres, p, grid, st);
+    case 32: return launch_bn<32, T>(ma, mw, ma2, mo, mres, p, grid, st);
+    case 16: return launch_bn<16, T>(ma, mw, ma2, mo, mres, p, grid, st);
+  })
   FYC_CHECK(false, "tensor-core GEMM: no kernel for BN = %d", p.BN);
 }
 
@@ -550,7 +554,7 @@ extern "C" int32_t fyc_tcgen05_available(void) { return get_encode_fn() != nullp
 
 // Is this GEMM eligible for the tensor-core path?
 bool fyc_gemm_tc_eligible(const fyc_gemm_args* g) {
-  if (g->dtype != FYC_BF16) return false;
+  if (!fyc_is_16bit(g->dtype)) return false;
   if (g->K % 8 || g->lda % 8 || g->ldw % 8 || g->N % 16 || g->M < 64) return false;
   if (((uintptr_t)g->A | (uintptr_t)g->W) & 15) return false;
   if (g->batch > 1 && ((g->strideA | g->strideW | g->strideO) % 8)) return false;
@@ -578,22 +582,22 @@ int32_t fyc_gemm_tc(const fyc_gemm_args* g, cudaStream_t st) {
   const bool geglu = (g->epilogue & FYC_EPI_GEGLU) != 0;
   const bool f32 = (g->epilogue & FYC_EPI_OUT_F32) != 0;
   for (int64_t b = 0; b < g->batch; ++b) {
-    const bf16* A = (const bf16*)g->A + b * g->strideA;
-    const bf16* W = (const bf16*)g->W + b * g->strideW;
+    const uint16_t* A = (const uint16_t*)g->A + b * g->strideA;     // 16-bit elements
+    const uint16_t* W = (const uint16_t*)g->W + b * g->strideW;
     CUtensorMap ma, mw, ma2;
     const int64_t Ka = g->A2 ? g->K1 : g->K;          // columns of the first (or only) source
     {
       uint64_t dims[4] = {(uint64_t)Ka, (uint64_t)g->M, 1, 1};
       uint64_t str[3] = {(uint64_t)g->lda * 2, (uint64_t)g->lda * 2 * (uint64_t)g->M, (uint64_t)g->lda * 2 * (uint64_t)g->M};
       uint32_t box[4] = {BK, BM, 1, 1};
-      int32_t rc = encode_map(&ma, A, 4, dims, str, box);
+      int32_t rc = encode_map(&ma, A, 4, dims, str, box, map_dtype(g->dtype));
       if (rc) return rc;
     }
     if (g->A2) {
       uint64_t dims[4] = {(uint64_t)(g->K - g->K1), (uint64_t)g->M, 1, 1};
       uint64_t str[3] = {(uint64_t)g->lda2 * 2, (uint64_t)g->lda2 * 2 * (uint64_t)g->M, (uint64_t)g->lda2 * 2 * (uint64_t)g->M};
       uint32_t box[4] = {BK, BM, 1, 1};
-      int32_t rc = encode_map(&ma2, g->A2, 4, dims, str, box);
+      int32_t rc = encode_map(&ma2, g->A2, 4, dims, str, box, map_dtype(g->dtype));
       if (rc) return rc;
     }
     TcParams p{};
@@ -609,7 +613,7 @@ int32_t fyc_gemm_tc(const fyc_gemm_args* g, cudaStream_t st) {
       uint64_t dims[3] = {(uint64_t)g->K, 1, (uint64_t)g->N};
       uint64_t str[2] = {(uint64_t)g->ldw * 2, (uint64_t)g->ldw * 2};
       uint32_t box[3] = {BK, 1, (uint32_t)p.BN};
-      int32_t rc = encode_map(&mw, W, 3, dims, str, box);
+      int32_t rc = encode_map(&mw, W, 3, dims, str, box, map_dtype(g->dtype));
       if (rc) return rc;
     }
     FYC_CHECK(g->M < (1ll << 31), "gemm(tensor cores): M too large");
@@ -621,13 +625,13 @@ int32_t fyc_gemm_tc(const fyc_gemm_args* g, cudaStream_t st) {
     const int64_t es = f32 ? 4 : 2;
     const uint64_t M = (uint64_t)g->M, No = (uint64_t)p.N_out;
     CUtensorMap mo, mr;
-    int32_t rc = encode_out_map(&mo, (const char*)g->out + b * g->strideO * es, p, No, M, 1, 1, g->ldo, g->ldo * M, g->ldo * M);
+    int32_t rc = encode_out_map(&mo, (const char*)g->out + b * g->strideO * es, p, g->dtype, No, M, 1, 1, g->ldo, g->ldo * M, g->ldo * M);
     if (rc) return rc;
     if (g->epilogue & FYC_EPI_RESIDUAL) {
-      rc = encode_out_map(&mr, (const char*)g->residual + b * g->strideO * es, p, No, M, 1, 1, g->ldr, g->ldr * M, g->ldr * M);
+      rc = encode_out_map(&mr, (const char*)g->residual + b * g->strideO * es, p, g->dtype, No, M, 1, 1, g->ldr, g->ldr * M, g->ldr * M);
       if (rc) return rc;
     }
-    rc = launch_tc(ma, mw, mo, (g->epilogue & FYC_EPI_RESIDUAL) ? &mr : nullptr, p, grid, st, g->A2 ? &ma2 : nullptr);
+    rc = launch_tc(g->dtype, ma, mw, mo, (g->epilogue & FYC_EPI_RESIDUAL) ? &mr : nullptr, p, grid, st, g->A2 ? &ma2 : nullptr);
     if (rc) return rc;
   }
   return FYC_OK;
@@ -644,7 +648,7 @@ static bool pick_patch(int64_t NB, int64_t Ho, int64_t Wo, int* bw, int* bh, int
 }
 
 bool fyc_conv3x3_tc_eligible(const fyc_conv3x3_args* c) {
-  if (c->dtype != FYC_BF16 || c->upsample != 1) return false;
+  if (!fyc_is_16bit(c->dtype) || c->upsample != 1) return false;
   if (c->stride != 1 && c->stride != 2) return false;
   if (c->Cin % 8 || c->Cout % 16) return false;
   if (c->stride == 2 && (c->H % 2 || c->W % 2)) return false;
@@ -692,14 +696,14 @@ int32_t fyc_conv3x3_tc(const fyc_conv3x3_args* c, const void* x_planes, cudaStre
     uint64_t dims[4] = {(uint64_t)c->Cin, (uint64_t)Wo, (uint64_t)Ho, imgs};
     uint64_t str[3] = {(uint64_t)c->Cin * 2, (uint64_t)c->Cin * 2 * Wo, (uint64_t)c->Cin * 2 * Wo * Ho};
     uint32_t box[4] = {BK, (uint32_t)p.bw, (uint32_t)p.bh, (uint32_t)p.bn};
-    int32_t rc = encode_map(&ma, xa, 4, dims, str, box);
+    int32_t rc = encode_map(&ma, xa, 4, dims, str, box, map_dtype(c->dtype));
     if (rc) return rc;
   }
   {
     uint64_t dims[3] = {(uint64_t)c->Cin, 9, (uint64_t)c->Cout};
     uint64_t str[2] = {(uint64_t)c->Cin * 2, (uint64_t)c->Cin * 2 * 9};
     uint32_t box[3] = {BK, 1, (uint32_t)p.BN};
-    int32_t rc = encode_map(&mw, c->w, 3, dims, str, box);
+    int32_t rc = encode_map(&mw, c->w, 3, dims, str, box, map_dtype(c->dtype));
     if (rc) return rc;
   }
   p.bias = c->bias; p.rowbias = c->rowbias;
@@ -708,13 +712,13 @@ int32_t fyc_conv3x3_tc(const fyc_conv3x3_args* c, const void* x_planes, cudaStre
   p.alpha = 1.0f;
   const uint64_t C = (uint64_t)c->Cout;
   CUtensorMap mo, mr;
-  int32_t rc = encode_out_map(&mo, c->out, p, C, Wo, Ho, c->NB, C, C * Wo, C * Wo * Ho);
+  int32_t rc = encode_out_map(&mo, c->out, p, c->dtype, C, Wo, Ho, c->NB, C, C * Wo, C * Wo * Ho);
   if (rc) return rc;
   if (c->epilogue & FYC_EPI_RESIDUAL) {
-    rc = encode_out_map(&mr, c->residual, p, C, Wo, Ho, c->NB, C, C * Wo, C * Wo * Ho);
+    rc = encode_out_map(&mr, c->residual, p, c->dtype, C, Wo, Ho, c->NB, C, C * Wo, C * Wo * Ho);
     if (rc) return rc;
   }
-  return launch_tc(ma, mw, mo, (c->epilogue & FYC_EPI_RESIDUAL) ? &mr : nullptr, p, grid, st);
+  return launch_tc(c->dtype, ma, mw, mo, (c->epilogue & FYC_EPI_RESIDUAL) ? &mr : nullptr, p, grid, st);
 }
 
 // nearest-x2 upsample + padded 3x3 conv as four 2x2-tap implicit GEMMs on the low-resolution image (fyc.h: w_phases).
@@ -724,7 +728,7 @@ int32_t fyc_conv3x3_tc(const fyc_conv3x3_args* c, const void* x_planes, cudaStre
 // {Cout, W, H, NB} with strides 2 Cout, 4W Cout, 4HW Cout elements, so low-resolution pixel (ow, oh, img) lands at
 // ((img * 2H + 2 oh + py) * 2W + 2 ow + px) * Cout, the NHWC offset of the upsampled pixel.
 bool fyc_conv3x3_up2_tc_eligible(const fyc_conv3x3_args* c) {
-  if (c->dtype != FYC_BF16 || c->upsample != 2 || c->stride != 1 || c->pad_mode != 0 || !c->w_phases) return false;
+  if (!fyc_is_16bit(c->dtype) || c->upsample != 2 || c->stride != 1 || c->pad_mode != 0 || !c->w_phases) return false;
   if (c->Cin % 8 || c->Cout % 16) return false;
   if (((uintptr_t)c->x | (uintptr_t)c->w_phases | (uintptr_t)c->out) & 15) return false;
   if (c->epilogue & ~FYC_EPI_BIAS) return false;          // the upsamplers carry a bias only (resnet.py:168, diffusers resnet.py:139)
@@ -752,7 +756,7 @@ int32_t fyc_conv3x3_up2_tc(const fyc_conv3x3_args* c, cudaStream_t st) {
     uint64_t dims[4] = {(uint64_t)c->Cin, (uint64_t)W, (uint64_t)H, (uint64_t)c->NB};
     uint64_t str[3] = {(uint64_t)c->Cin * 2, (uint64_t)c->Cin * 2 * W, (uint64_t)c->Cin * 2 * W * H};
     uint32_t box[4] = {BK, (uint32_t)p.bw, (uint32_t)p.bh, (uint32_t)p.bn};
-    int32_t rc = encode_map(&ma, c->x, 4, dims, str, box);
+    int32_t rc = encode_map(&ma, c->x, 4, dims, str, box, map_dtype(c->dtype));
     if (rc) return rc;
   }
   for (int ph = 0; ph < 4; ++ph) {
@@ -761,17 +765,17 @@ int32_t fyc_conv3x3_up2_tc(const fyc_conv3x3_args* c, cudaStream_t st) {
       p.tap_dy[t] = (t >> 1) - 1 + py; p.tap_dx[t] = (t & 1) - 1 + px; p.tap_img[t] = 0;
     }
     CUtensorMap mw;
-    const bf16* wp = (const bf16*)c->w_phases + (int64_t)ph * c->Cout * 4 * c->Cin;
+    const uint16_t* wp = (const uint16_t*)c->w_phases + (int64_t)ph * c->Cout * 4 * c->Cin;
     uint64_t dims[3] = {(uint64_t)c->Cin, 4, (uint64_t)c->Cout};
     uint64_t str[2] = {(uint64_t)c->Cin * 2, (uint64_t)c->Cin * 2 * 4};
     uint32_t box[3] = {BK, 1, (uint32_t)p.BN};
-    int32_t rc = encode_map(&mw, wp, 3, dims, str, box);
+    int32_t rc = encode_map(&mw, wp, 3, dims, str, box, map_dtype(c->dtype));
     if (rc) return rc;
     const uint64_t C = (uint64_t)c->Cout;
     CUtensorMap mo;
-    rc = encode_out_map(&mo, (const bf16*)c->out + ((int64_t)py * 2 * W + px) * c->Cout, p, C, W, H, c->NB, 2 * C, 4 * W * C, 4 * H * W * C);
+    rc = encode_out_map(&mo, (const uint16_t*)c->out + ((int64_t)py * 2 * W + px) * c->Cout, p, c->dtype, C, W, H, c->NB, 2 * C, 4 * W * C, 4 * H * W * C);
     if (rc) return rc;
-    rc = launch_tc(ma, mw, mo, nullptr, p, grid, st);
+    rc = launch_tc(c->dtype, ma, mw, mo, nullptr, p, grid, st);
     if (rc) return rc;
   }
   return FYC_OK;

@@ -28,17 +28,20 @@ static int fyc_gn_waves() {
 }
 
 namespace {
-// one 32-bit word holding two bf16 <-> two floats (element 0 in the low half); a 16-byte vector of eight <-> float[8]
-__device__ __forceinline__ void bf2_to_f2(uint32_t w, float& lo, float& hi) { lo = __uint_as_float(w << 16); hi = __uint_as_float(w & 0xffff0000u); }
-__device__ __forceinline__ uint32_t f2_to_bf2(float lo, float hi) {
-  __nv_bfloat162 h = __floats2bfloat162_rn(lo, hi);
-  return *reinterpret_cast<uint32_t*>(&h);
+// one 32-bit word holding two 16-bit T (bf16 | f16) <-> two floats (element 0 in the low half); a 16-byte vector of eight <-> float[8]
+template <typename T> __device__ __forceinline__ void u2_to_f2(uint32_t w, float& lo, float& hi) {
+  if constexpr (std::is_same<T, bf16>::value) {
+    lo = __uint_as_float(w << 16); hi = __uint_as_float(w & 0xffff0000u);
+  } else {
+    const float2 f = Pair16<T>::unpack(*reinterpret_cast<const typename Pair16<T>::type*>(&w));
+    lo = f.x; hi = f.y;
+  }
 }
-__device__ __forceinline__ void bf8_to_f(const uint4& raw, float* f) {
-  bf2_to_f2(raw.x, f[0], f[1]); bf2_to_f2(raw.y, f[2], f[3]); bf2_to_f2(raw.z, f[4], f[5]); bf2_to_f2(raw.w, f[6], f[7]);
+template <typename T> __device__ __forceinline__ void u8_to_f(const uint4& raw, float* f) {
+  u2_to_f2<T>(raw.x, f[0], f[1]); u2_to_f2<T>(raw.y, f[2], f[3]); u2_to_f2<T>(raw.z, f[4], f[5]); u2_to_f2<T>(raw.w, f[6], f[7]);
 }
-__device__ __forceinline__ uint4 f_to_bf8(const float* f) {
-  return make_uint4(f2_to_bf2(f[0], f[1]), f2_to_bf2(f[2], f[3]), f2_to_bf2(f[4], f[5]), f2_to_bf2(f[6], f[7]));
+template <typename T> __device__ __forceinline__ uint4 f_to_u8(const float* f) {
+  return make_uint4(pack_u32<T>(f[0], f[1]), pack_u32<T>(f[2], f[3]), pack_u32<T>(f[4], f[5]), pack_u32<T>(f[6], f[7]));
 }
 // four fp32 parameters with one 16-byte load (scalar parameter loads saturated the LSU queue: lg_throttle)
 __device__ __forceinline__ void ldg4(const float* p, float* f) {
@@ -80,7 +83,7 @@ __global__ void __launch_bounds__(256, 4) gn_stats_kernel(const T* __restrict__ 
       for (int e = 0; e < V; ++e) { s[e] = 0.f; q[e] = 0.f; }
       int64_t r = r0 + ry;
       if constexpr (sizeof(T) == 2 && V == 8) {
-        // bf16: 8 independent 16-byte loads in flight per thread, kept as bf16 until they are summed (the 4-deep version was
+        // 16-bit: 8 independent 16-byte loads in flight per thread, kept packed until they are summed (the 4-deep version was
         // latency-bound: long-scoreboard stalls)
         for (; r + 7 * RY < r1; r += 8 * RY) {
           uint4 raw[8];
@@ -89,7 +92,7 @@ __global__ void __launch_bounds__(256, 4) gn_stats_kernel(const T* __restrict__ 
 #pragma unroll
           for (int u = 0; u < 8; ++u) {
             float f[8];
-            bf8_to_f(raw[u], f);
+            u8_to_f<T>(raw[u], f);
 #pragma unroll
             for (int e = 0; e < 8; ++e) { s[e] = __fadd_rn(s[e], f[e]); q[e] = __fmaf_rn(f[e], f[e], q[e]); }
           }
@@ -217,7 +220,7 @@ __global__ void __launch_bounds__(256) gn_apply_kernel(const T* __restrict__ x, 
   }
 }
 
-// bf16 apply, second form: a thread owns ONE 8-channel vector (scale / shift live in 16 registers, loaded once) and walks rows,
+// 16-bit apply, second form: a thread owns ONE 8-channel vector (scale / shift live in 16 registers, loaded once) and walks rows,
 // U rows in flight.  The grid-stride form above re-derived (image, channel) and re-loaded four
 // parameter vectors for every 16 bytes of data: 160 issued instructions per vector, 51 us for an 84 MB tensor.
 // [r2] Row blocks (RY x U consecutive rows) are dealt to the CTAs round-robin - neighbouring CTAs stream neighbouring memory at the same
@@ -226,10 +229,10 @@ __global__ void __launch_bounds__(256) gn_apply_kernel(const T* __restrict__ x, 
 // element instead of EX2 + RCP (the apply kernel spent a third of its issue slots and all of its MUFU slots there).
 __device__ __forceinline__ float tanh_fast(float x) { float y; asm("tanh.approx.f32 %0, %1;" : "=f"(y) : "f"(x)); return y; }
 
-template <bool SILU>
-__global__ void __launch_bounds__(256, 3) gn_apply_rows_kernel(const bf16* __restrict__ x, const float* __restrict__ scale,
-                                                            const float* __restrict__ shift, bf16* __restrict__ out, int64_t R,
-                                                            int C, const bf16* __restrict__ x2, int C1) {
+template <typename T, bool SILU>
+__global__ void __launch_bounds__(256, 3) gn_apply_rows_kernel(const T* __restrict__ x, const float* __restrict__ scale,
+                                                            const float* __restrict__ shift, T* __restrict__ out, int64_t R,
+                                                            int C, const T* __restrict__ x2, int C1) {
   constexpr int U = 4;
   const int cvn = C / 8;
   const int TX = cvn < 256 ? cvn : 256;
@@ -239,11 +242,11 @@ __global__ void __launch_bounds__(256, 3) gn_apply_rows_kernel(const bf16* __res
   const int64_t nb = blockIdx.y;
   const int64_t blk_rows = (int64_t)RY * U;                     // rows one CTA iteration covers
   const int64_t nblk = (R + blk_rows - 1) / blk_rows;
-  bf16* ob = out + nb * R * C;
+  T* ob = out + nb * R * C;
   for (int cv = tx; cv < cvn; cv += TX) {
     const bool second = x2 != nullptr && cv * 8 >= C1;
     const int ldx = x2 == nullptr ? C : (second ? C - C1 : C1);
-    const bf16* xb = second ? x2 + nb * R * ldx + (cv * 8 - C1) : x + nb * R * ldx + cv * 8;     // row r of this channel vector: xb + r * ldx
+    const T* xb = second ? x2 + nb * R * ldx + (cv * 8 - C1) : x + nb * R * ldx + cv * 8;     // row r of this channel vector: xb + r * ldx
     float sc[8], sh[8];
     ldg4(scale + nb * C + cv * 8, sc); ldg4(scale + nb * C + cv * 8 + 4, sc + 4);
     ldg4(shift + nb * C + cv * 8, sh); ldg4(shift + nb * C + cv * 8 + 4, sh + 4);
@@ -269,13 +272,13 @@ __global__ void __launch_bounds__(256, 3) gn_apply_rows_kernel(const bf16* __res
 #pragma unroll
         for (int e = 0; e < 4; ++e) {
           float y0, y1;
-          bf2_to_f2(w[e], y0, y1);
+          u2_to_f2<T>(w[e], y0, y1);
           y0 = __fmaf_rn(y0, sc[2 * e], sh[2 * e]); y1 = __fmaf_rn(y1, sc[2 * e + 1], sh[2 * e + 1]);
           if (SILU) {                       // y * sigmoid(y) = y * (0.5 + 0.5 tanh(y / 2))
             const float h0 = __fmul_rn(y0, 0.5f), h1 = __fmul_rn(y1, 0.5f);
             y0 = __fmul_rn(y0, __fmaf_rn(tanh_fast(h0), 0.5f, 0.5f)); y1 = __fmul_rn(y1, __fmaf_rn(tanh_fast(h1), 0.5f, 0.5f));
           }
-          o[e] = f2_to_bf2(y0, y1);
+          o[e] = pack_u32<T>(y0, y1);
         }
         *reinterpret_cast<uint4*>(ob + rr * C + cv * 8) = make_uint4(o[0], o[1], o[2], o[3]);
       }
@@ -323,8 +326,8 @@ static int32_t groupnorm_impl(const T* x, const float* gamma, const float* beta,
     const int64_t nblk = ceil_div64(R, (int64_t)RY * 4);
     if (want > nblk) want = nblk;
     dim3 ga((unsigned)want, (unsigned)NB);
-    if (silu) gn_apply_rows_kernel<true><<<ga, 256, 0, st>>>((const bf16*)x, scale, shift, (bf16*)out, R, C, (const bf16*)x2, C1);
-    else gn_apply_rows_kernel<false><<<ga, 256, 0, st>>>((const bf16*)x, scale, shift, (bf16*)out, R, C, (const bf16*)x2, C1);
+    if (silu) gn_apply_rows_kernel<T, true><<<ga, 256, 0, st>>>(x, scale, shift, out, R, C, x2, C1);
+    else gn_apply_rows_kernel<T, false><<<ga, 256, 0, st>>>(x, scale, shift, out, R, C, x2, C1);
     FYC_LAUNCH_CHECK();
     return FYC_OK;
   }
@@ -351,9 +354,11 @@ extern "C" int32_t fyc_groupnorm(const void* x, const float* gamma, const float*
                                  size_t workspace_bytes, void* stream) {
   if (const int32_t err = gn_check_args("groupnorm", NB, R, C, G, workspace, workspace_bytes)) return err;
   cudaStream_t st = (cudaStream_t)stream;
-  if (dtype == FYC_BF16) {
-    if (C % 8 == 0) return groupnorm_impl<bf16, 8>((const bf16*)x, gamma, beta, (bf16*)out, NB, R, (int)C, (int)G, eps, silu, workspace, st);
-    return groupnorm_impl<bf16, 1>((const bf16*)x, gamma, beta, (bf16*)out, NB, R, (int)C, (int)G, eps, silu, workspace, st);
+  if (fyc_is_16bit(dtype)) {
+    FYC_DISPATCH16(dtype, {
+      if (C % 8 == 0) return groupnorm_impl<T, 8>((const T*)x, gamma, beta, (T*)out, NB, R, (int)C, (int)G, eps, silu, workspace, st);
+      return groupnorm_impl<T, 1>((const T*)x, gamma, beta, (T*)out, NB, R, (int)C, (int)G, eps, silu, workspace, st);
+    })
   } else if (dtype == FYC_F32) {
     if (C % 4 == 0) return groupnorm_impl<float, 4>((const float*)x, gamma, beta, (float*)out, NB, R, (int)C, (int)G, eps, silu, workspace, st);
     return groupnorm_impl<float, 1>((const float*)x, gamma, beta, (float*)out, NB, R, (int)C, (int)G, eps, silu, workspace, st);
@@ -368,9 +373,9 @@ extern "C" int32_t fyc_groupnorm_concat(const void* x1, int64_t C1, const void* 
   FYC_CHECK(x1 && x2 && C1 > 0 && C2 > 0, "groupnorm_concat: bad arguments");
   if (const int32_t err = gn_check_args("groupnorm_concat", NB, R, C, G, workspace, workspace_bytes)) return err;
   cudaStream_t st = (cudaStream_t)stream;
-  if (dtype == FYC_BF16) {
+  if (fyc_is_16bit(dtype)) {
     FYC_CHECK(C1 % 8 == 0 && C2 % 8 == 0 && ((((uintptr_t)x1 | (uintptr_t)x2 | (uintptr_t)out)) & 15) == 0, "groupnorm_concat(bf16): channel counts must be multiples of 8, pointers 16-byte aligned");
-    return groupnorm_impl<bf16, 8>((const bf16*)x1, gamma, beta, (bf16*)out, NB, R, (int)C, (int)G, eps, silu, workspace, st, (const bf16*)x2, (int)C1);
+    FYC_DISPATCH16(dtype, return groupnorm_impl<T, 8>((const T*)x1, gamma, beta, (T*)out, NB, R, (int)C, (int)G, eps, silu, workspace, st, (const T*)x2, (int)C1))
   } else if (dtype == FYC_F32) {
     FYC_CHECK(C1 % 4 == 0 && C2 % 4 == 0, "groupnorm_concat(f32): channel counts must be multiples of 4");
     return groupnorm_impl<float, 4>((const float*)x1, gamma, beta, (float*)out, NB, R, (int)C, (int)G, eps, silu, workspace, st, (const float*)x2, (int)C1);
@@ -410,13 +415,13 @@ __device__ __forceinline__ void ln_warp_row_stats(const T* xr, int lane, int cvn
 // LPR form (layernorm_lpr_kernel, ln_stats_lpr_kernel): LPR lanes share a row of C = 40 * LPR channels, five 16-byte vectors per
 // lane.  From a lane's raw vectors to the centred values v, the row's mean and rstd: two-pass, even and odd elements accumulated
 // separately, combined over the row's lanes by xor-shuffle - every lane of the warp must take part.
-template <int LPR>
+template <typename T, int LPR>
 __device__ __forceinline__ void ln_lpr_row_stats(const uint4 (&raw)[5], float eps, float (&v)[5][8], float& mean, float& rstd) {
   const float inv_c = 1.0f / (float)(LPR * 40);
   float s0 = 0.f, s1 = 0.f;
 #pragma unroll
   for (int i = 0; i < 5; ++i) {
-    bf8_to_f(raw[i], v[i]);
+    u8_to_f<T>(raw[i], v[i]);
 #pragma unroll
     for (int e = 0; e < 8; e += 2) { s0 = __fadd_rn(s0, v[i][e]); s1 = __fadd_rn(s1, v[i][e + 1]); }
   }
@@ -474,13 +479,13 @@ __global__ void __launch_bounds__(256) layernorm_kernel(const T* __restrict__ x,
   }
 }
 
-// bf16 LayerNorm, RPW rows per warp: every row's 16-byte vectors are requested before any is used (RPW x NV loads in
+// 16-bit LayerNorm, RPW rows per warp: every row's 16-byte vectors are requested before any is used (RPW x NV loads in
 // flight per lane instead of NV), gamma / beta are read once per warp instead of once per row.  The one-row kernel ran at
 // 2.6 TB/s of the 6.6 TB/s the copy benchmark reaches: too few bytes in flight per SM and ~5 parameter loads per data load.
 // (Its statistics multiply by 1 / C where the warp-per-row pair divides by C: it has no statistics-only twin to agree with.)
-template <int NV, int RPW>
-__global__ void __launch_bounds__(256) layernorm_bf16_kernel(const bf16* __restrict__ x, const float* __restrict__ gamma,
-                                                             const float* __restrict__ beta, bf16* __restrict__ out, int64_t M,
+template <typename T, int NV, int RPW>
+__global__ void __launch_bounds__(256) layernorm_rows_kernel(const T* __restrict__ x, const float* __restrict__ gamma,
+                                                             const float* __restrict__ beta, T* __restrict__ out, int64_t M,
                                                              int C, float eps, const float* __restrict__ pe,
                                                              int64_t rows_per_frame, int64_t frames) {
   const int lane = threadIdx.x & 31;
@@ -514,7 +519,7 @@ __global__ void __launch_bounds__(256) layernorm_bf16_kernel(const bf16* __restr
     float sum = 0.f;
 #pragma unroll
     for (int i = 0; i < NV; ++i) {
-      bf8_to_f(raw[r][i], v[i]);
+      u8_to_f<T>(raw[r][i], v[i]);
       if (lane + 32 * i < cvn) {
 #pragma unroll
         for (int e = 0; e < 8; ++e) sum += v[i][e];
@@ -538,20 +543,20 @@ __global__ void __launch_bounds__(256) layernorm_bf16_kernel(const bf16* __restr
         if (per) { ldg4(per + cv * 8, pb); ldg4(per + cv * 8 + 4, pb + 4); }
 #pragma unroll
         for (int e = 0; e < 8; ++e) o[e] = (v[i][e] - mean) * rstd * gm[i][e] + (bt[i][e] + pb[e]);
-        Vec8<bf16>::store(out + row * C + cv * 8, o);
+        Vec8<T>::store(out + row * C + cv * 8, o);
       }
     }
   }
 }
 
-// bf16 LayerNorm for C = 40 * LPR (320 / 640 / 1280): LPR lanes share a row, five 16-byte vectors per lane - every lane is busy
+// 16-bit LayerNorm for C = 40 * LPR (320 / 640 / 1280): LPR lanes share a row, five 16-byte vectors per lane - every lane is busy
 // (the warp-per-row kernels idle 24 of 32 lanes on the second vector of a 320-wide row), 32 / LPR rows per warp pass, PASSES passes
 // with all loads of a pass issued up front.  gamma stays in registers for the warp's lifetime; the arithmetic is the same
 // two-pass (mean, then centred variance) as the reference kernel in explicitly rounded, never contracted fp32 steps: ~5 issued
 // instructions per element instead of ~18.
-template <int LPR, int PASSES, bool HAS_PE>
-__global__ void __launch_bounds__(256, 2) layernorm_lpr_kernel(const bf16* __restrict__ x, const float* __restrict__ gamma,
-                                                               const float* __restrict__ beta, bf16* __restrict__ out, int64_t M,
+template <typename T, int LPR, int PASSES, bool HAS_PE>
+__global__ void __launch_bounds__(256, 2) layernorm_lpr_kernel(const T* __restrict__ x, const float* __restrict__ gamma,
+                                                               const float* __restrict__ beta, T* __restrict__ out, int64_t M,
                                                                float eps, const float* __restrict__ pe, int64_t rows_per_frame,
                                                                int64_t frames, int rev) {
   constexpr int C = LPR * 40, RPP = 32 / LPR;           // channels; rows per warp pass
@@ -572,14 +577,14 @@ __global__ void __launch_bounds__(256, 2) layernorm_lpr_kernel(const bf16* __res
     const int64_t row = row_base + ps * RPP + rr;
     const bool ok = row < M;
     const int64_t rowc = ok ? row : M - 1;            // out-of-range lanes shadow the last row (shuffles stay full-warp), never store
-    const bf16* xr = x + rowc * C + sub * 8;
+    const T* xr = x + rowc * C + sub * 8;
     uint4 raw[5];
 #pragma unroll
     for (int i = 0; i < 5; ++i) raw[i] = __ldg(reinterpret_cast<const uint4*>(xr + i * VS));
     float v[5][8], mean, rstd;
-    ln_lpr_row_stats<LPR>(raw, eps, v, mean, rstd);
+    ln_lpr_row_stats<T, LPR>(raw, eps, v, mean, rstd);
     const float* pp = HAS_PE ? pe + ((rowc / rows_per_frame) % frames) * C + sub * 8 : nullptr;
-    bf16* orow = out + rowc * C + sub * 8;
+    T* orow = out + rowc * C + sub * 8;
 #pragma unroll
     for (int i = 0; i < 5; ++i) {
       float bb[8], o[8];
@@ -592,27 +597,32 @@ __global__ void __launch_bounds__(256, 2) layernorm_lpr_kernel(const bf16* __res
       }
 #pragma unroll
       for (int e = 0; e < 8; ++e) o[e] = __fmaf_rn(__fmul_rn(v[i][e], rstd), gm[i][e], bb[e]);
-      const uint4 packed = f_to_bf8(o);
+      const uint4 packed = f_to_u8<T>(o);
       if (ok) *reinterpret_cast<uint4*>(orow + i * VS) = packed;
     }
   }
 }
 
-// LayerNorm STATISTICS only (fyc_layernorm_stats): per row rstd (fp32) and the 8-column bf16 "aug" row [m_hi, m_hi, m_lo, m_lo, 0, 0, 0, 0]
+// LayerNorm STATISTICS only (fyc_layernorm_stats): per row rstd (fp32) and the 8-column 16-bit "aug" row [m_hi, m_hi, m_lo, m_lo, 0, 0, 0, 0]
 // (mean = m_hi + m_lo) that the LN-folded GEMM appends to its K dimension (fyc.h FYC_EPI_LNFOLD).  Same lane layout and the same
 // row statistics as layernorm_lpr_kernel - one read of x, no write of a normalised copy.  PASSES x 5 independent 16-byte loads
 // per lane are requested before the first is used.
-__device__ __forceinline__ void ln_write_stats(float* __restrict__ rstd_out, bf16* __restrict__ aug, int64_t row, float mean, float rstd) {
+// AT: the aug element type.  bf16: hi + lo keeps 16 significand bits of the mean (relative error <= 2^-17).  fp16: hi + lo keeps 22
+// bits while m_lo is a normal number (|mean| >= 2^-3); below that m_lo is subnormal and the absolute error stays <= 2^-25, which is
+// <= 2^-17 |mean| for every |mean| >= 2^-8 - so the fp16 pair is at least as exact as the bf16 one except for means under 0.004, where
+// it is off by at most 3e-8.  |mean| never exceeds the fp16 range: it averages fp16 values.
+template <typename AT>
+__device__ __forceinline__ void ln_write_stats(float* __restrict__ rstd_out, AT* __restrict__ aug, int64_t row, float mean, float rstd) {
   rstd_out[row] = rstd;
   if (aug == nullptr) return;
-  const bf16 hi = __float2bfloat16_rn(mean);
-  const bf16 lo = __float2bfloat16_rn(mean - __bfloat162float(hi));
-  const uint32_t hh = (uint32_t)__bfloat16_as_ushort(hi) * 0x10001u, ll = (uint32_t)__bfloat16_as_ushort(lo) * 0x10001u;
+  const AT hi = from_f<AT>(mean);
+  const AT lo = from_f<AT>(mean - to_f(hi));
+  const uint32_t hh = (uint32_t)*reinterpret_cast<const uint16_t*>(&hi) * 0x10001u, ll = (uint32_t)*reinterpret_cast<const uint16_t*>(&lo) * 0x10001u;
   *reinterpret_cast<uint4*>(aug + row * 8) = make_uint4(hh, ll, 0u, 0u);
 }
 
-template <int LPR, int PASSES>
-__global__ void __launch_bounds__(256, 2) ln_stats_lpr_kernel(const bf16* __restrict__ x, float* __restrict__ rstd_out, bf16* __restrict__ aug,
+template <typename T, int LPR, int PASSES>
+__global__ void __launch_bounds__(256, 2) ln_stats_lpr_kernel(const T* __restrict__ x, float* __restrict__ rstd_out, T* __restrict__ aug,
                                                               int64_t M, float eps, int rev) {
   constexpr int C = LPR * 40, RPP = 32 / LPR, VS = LPR * 8;
   const int lane = threadIdx.x & 31, sub = lane % LPR, rr = lane / LPR;
@@ -624,7 +634,7 @@ __global__ void __launch_bounds__(256, 2) ln_stats_lpr_kernel(const bf16* __rest
   for (int ps = 0; ps < PASSES; ++ps) {
     const int64_t row = row_base + ps * RPP + rr;
     const int64_t rowc = row < M ? row : M - 1;       // out-of-range lanes shadow the last row (shuffles stay full-warp), never store
-    const bf16* xr = x + rowc * C + sub * 8;
+    const T* xr = x + rowc * C + sub * 8;
 #pragma unroll
     for (int i = 0; i < 5; ++i) raw[ps][i] = __ldg(reinterpret_cast<const uint4*>(xr + i * VS));
   }
@@ -632,14 +642,14 @@ __global__ void __launch_bounds__(256, 2) ln_stats_lpr_kernel(const bf16* __rest
   for (int ps = 0; ps < PASSES; ++ps) {
     const int64_t row = row_base + ps * RPP + rr;
     float v[5][8], mean, rstd;
-    ln_lpr_row_stats<LPR>(raw[ps], eps, v, mean, rstd);
+    ln_lpr_row_stats<T, LPR>(raw[ps], eps, v, mean, rstd);
     if (sub == 0 && row < M) ln_write_stats(rstd_out, aug, row, mean, rstd);
   }
 }
 
-// generic widths (C % 8 == 0, C <= 2048; bf16) and fp32 rows: one warp per row
-template <typename T, int V, int NV>
-__global__ void __launch_bounds__(256) ln_stats_kernel(const T* __restrict__ x, float* __restrict__ rstd_out, bf16* __restrict__ aug, int64_t M, int C, float eps) {
+// generic widths (C % 8 == 0, C <= 2048; 16-bit) and fp32 rows (bf16 aug): one warp per row
+template <typename T, int V, int NV, typename AT>
+__global__ void __launch_bounds__(256) ln_stats_kernel(const T* __restrict__ x, float* __restrict__ rstd_out, AT* __restrict__ aug, int64_t M, int C, float eps) {
   const int lane = threadIdx.x & 31;
   const int64_t row = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
   if (row >= M) return;
@@ -650,7 +660,7 @@ __global__ void __launch_bounds__(256) ln_stats_kernel(const T* __restrict__ x, 
 }
 
 // The row-width classes of fyc_layernorm and fyc_layernorm_stats (C already checked: a multiple of V, <= 2048): calls
-// f(LPR, NV) with compile-time constants - LPR != 0: an LPR kernel (bf16, C = 40 * LPR); LPR == 0: a warp-per-row kernel with
+// f(LPR, NV) with compile-time constants - LPR != 0: an LPR kernel (16-bit, C = 40 * LPR); LPR == 0: a warp-per-row kernel with
 // NV vectors of V = 16 / sizeof(T) elements per lane.
 template <int N> using int_c = std::integral_constant<int, N>;
 template <typename T, typename F>
@@ -668,14 +678,14 @@ static void ln_for_width(int64_t C, F f) {
   }
 }
 
-template <typename T>
-static void layernorm_stats_launch(const T* x, float* rstd, bf16* aug, int64_t M, int64_t C, float eps, cudaStream_t st) {
+template <typename T, typename AT>
+static void layernorm_stats_launch(const T* x, float* rstd, AT* aug, int64_t M, int64_t C, float eps, cudaStream_t st) {
   ln_for_width<T>(C, [&](auto lpr, auto nv) {
     constexpr int LPR = decltype(lpr)::value, NV = decltype(nv)::value, PASSES = 4;
     if constexpr (LPR != 0)
-      ln_stats_lpr_kernel<LPR, PASSES><<<(unsigned)ceil_div64(M, 8 * (32 / LPR) * PASSES), 256, 0, st>>>(x, rstd, aug, M, eps, fyc_zigzag());
+      ln_stats_lpr_kernel<T, LPR, PASSES><<<(unsigned)ceil_div64(M, 8 * (32 / LPR) * PASSES), 256, 0, st>>>(x, rstd, aug, M, eps, fyc_zigzag());
     else
-      ln_stats_kernel<T, 16 / sizeof(T), NV><<<(unsigned)ceil_div64(M, 8), 256, 0, st>>>(x, rstd, aug, M, (int)C, eps);
+      ln_stats_kernel<T, 16 / sizeof(T), NV, AT><<<(unsigned)ceil_div64(M, 8), 256, 0, st>>>(x, rstd, aug, M, (int)C, eps);
   });
 }
 
@@ -683,9 +693,9 @@ extern "C" int32_t fyc_layernorm_stats(const void* x, float* rstd, void* aug, in
   cudaStream_t st = (cudaStream_t)stream;
   FYC_CHECK(x && rstd && M > 0 && C > 0, "layernorm_stats: bad arguments");
   FYC_CHECK((((uintptr_t)x | (uintptr_t)aug) & 15) == 0 && (((uintptr_t)rstd) & 3) == 0, "layernorm_stats: alignment");
-  if (dtype == FYC_BF16) {
+  if (fyc_is_16bit(dtype)) {
     FYC_CHECK(C % 8 == 0 && C <= 2048, "layernorm_stats(bf16): C=%lld must be a multiple of 8 and <= 2048", (long long)C);
-    layernorm_stats_launch((const bf16*)x, rstd, (bf16*)aug, M, C, eps, st);
+    FYC_DISPATCH16(dtype, layernorm_stats_launch((const T*)x, rstd, (T*)aug, M, C, eps, st))
   } else if (dtype == FYC_F32) {
     FYC_CHECK(C % 4 == 0 && C <= 2048, "layernorm_stats(f32): C=%lld must be a multiple of 4 and <= 2048", (long long)C);
     layernorm_stats_launch((const float*)x, rstd, (bf16*)aug, M, C, eps, st);
@@ -703,12 +713,12 @@ static void layernorm_launch(const T* x, const float* gamma, const float* beta, 
     constexpr int LPR = decltype(lpr)::value, NV = decltype(nv)::value, PASSES = 2;
     if constexpr (LPR != 0) {
       const unsigned grid = (unsigned)ceil_div64(M, 8 * (32 / LPR) * PASSES);
-      if (pe) layernorm_lpr_kernel<LPR, PASSES, true><<<grid, 256, 0, st>>>(x, gamma, beta, out, M, eps, pe, rows_per_frame, frames, fyc_zigzag());
-      else layernorm_lpr_kernel<LPR, PASSES, false><<<grid, 256, 0, st>>>(x, gamma, beta, out, M, eps, pe, rows_per_frame, frames, fyc_zigzag());
+      if (pe) layernorm_lpr_kernel<T, LPR, PASSES, true><<<grid, 256, 0, st>>>(x, gamma, beta, out, M, eps, pe, rows_per_frame, frames, fyc_zigzag());
+      else layernorm_lpr_kernel<T, LPR, PASSES, false><<<grid, 256, 0, st>>>(x, gamma, beta, out, M, eps, pe, rows_per_frame, frames, fyc_zigzag());
     } else {
-      if constexpr (sizeof(T) == 2) {       // narrow bf16 rows: several rows per warp
-        if (C <= 8 * 32 * 2) return layernorm_bf16_kernel<2, 4><<<(unsigned)ceil_div64(M, 8 * 4), 256, 0, st>>>(x, gamma, beta, out, M, (int)C, eps, pe, rows_per_frame, frames);
-        if (C <= 8 * 32 * 3) return layernorm_bf16_kernel<3, 2><<<(unsigned)ceil_div64(M, 8 * 2), 256, 0, st>>>(x, gamma, beta, out, M, (int)C, eps, pe, rows_per_frame, frames);
+      if constexpr (sizeof(T) == 2) {       // narrow 16-bit rows: several rows per warp
+        if (C <= 8 * 32 * 2) return layernorm_rows_kernel<T, 2, 4><<<(unsigned)ceil_div64(M, 8 * 4), 256, 0, st>>>(x, gamma, beta, out, M, (int)C, eps, pe, rows_per_frame, frames);
+        if (C <= 8 * 32 * 3) return layernorm_rows_kernel<T, 3, 2><<<(unsigned)ceil_div64(M, 8 * 2), 256, 0, st>>>(x, gamma, beta, out, M, (int)C, eps, pe, rows_per_frame, frames);
       }
       layernorm_kernel<T, 16 / sizeof(T), NV><<<(unsigned)ceil_div64(M, 8), 256, 0, st>>>(x, gamma, beta, out, M, (int)C, eps, pe, rows_per_frame, frames);
     }
@@ -721,10 +731,10 @@ extern "C" int32_t fyc_layernorm(const void* x, const float* gamma, const float*
   cudaStream_t st = (cudaStream_t)stream;
   FYC_CHECK(M > 0 && C > 0, "layernorm: bad shape");
   if (pe) FYC_CHECK(rows_per_frame > 0 && frames > 0, "layernorm: pe needs rows_per_frame/frames");
-  if (dtype == FYC_BF16) {
+  if (fyc_is_16bit(dtype)) {
     FYC_CHECK(C % 8 == 0 && C <= 8 * 32 * 8, "layernorm(bf16): C=%lld must be a multiple of 8 and <= 2048", (long long)C);
     FYC_CHECK((((uintptr_t)x | (uintptr_t)out) & 15) == 0 && (((uintptr_t)gamma | (uintptr_t)beta | (uintptr_t)pe) & 15) == 0, "layernorm(bf16): 16-byte alignment");
-    layernorm_launch((const bf16*)x, gamma, beta, (bf16*)out, M, C, eps, pe, rows_per_frame, frames, st);
+    FYC_DISPATCH16(dtype, layernorm_launch((const T*)x, gamma, beta, (T*)out, M, C, eps, pe, rows_per_frame, frames, st))
   } else if (dtype == FYC_F32) {
     FYC_CHECK(C % 4 == 0 && C <= 4 * 32 * 16, "layernorm(f32): C=%lld must be a multiple of 4 and <= 2048", (long long)C);
     layernorm_launch((const float*)x, gamma, beta, (float*)out, M, C, eps, pe, rows_per_frame, frames, st);

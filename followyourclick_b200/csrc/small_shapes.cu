@@ -111,12 +111,15 @@ int32_t fyc_gemv(const fyc_gemm_args* g, cudaStream_t st) {
   if (g->dtype == FYC_F32) {
     gemv_small_m_kernel<float, float, 8><<<grid, 256, 0, st>>>((const float*)g->A, (const float*)g->W, (float*)g->out, (int)g->M, g->N, g->K,
                                                                  g->lda, g->ldw, g->ldo, bias, (const float*)res, g->ldr, g->alpha);
-  } else if (f32out) {
-    gemv_small_m_kernel<bf16, float, 8><<<grid, 256, 0, st>>>((const bf16*)g->A, (const bf16*)g->W, (float*)g->out, (int)g->M, g->N, g->K,
-                                                                g->lda, g->ldw, g->ldo, bias, (const float*)res, g->ldr, g->alpha);
   } else {
-    gemv_small_m_kernel<bf16, bf16, 8><<<grid, 256, 0, st>>>((const bf16*)g->A, (const bf16*)g->W, (bf16*)g->out, (int)g->M, g->N, g->K,
-                                                               g->lda, g->ldw, g->ldo, bias, (const bf16*)res, g->ldr, g->alpha);
+    FYC_DISPATCH16(g->dtype, {
+      if (f32out)
+        gemv_small_m_kernel<T, float, 8><<<grid, 256, 0, st>>>((const T*)g->A, (const T*)g->W, (float*)g->out, (int)g->M, g->N, g->K,
+                                                               g->lda, g->ldw, g->ldo, bias, (const float*)res, g->ldr, g->alpha);
+      else
+        gemv_small_m_kernel<T, T, 8><<<grid, 256, 0, st>>>((const T*)g->A, (const T*)g->W, (T*)g->out, (int)g->M, g->N, g->K,
+                                                           g->lda, g->ldw, g->ldo, bias, (const T*)res, g->ldr, g->alpha);
+    })
   }
   FYC_LAUNCH_CHECK();
   return FYC_OK;
@@ -130,6 +133,9 @@ bool fyc_conv_small_n_eligible(const fyc_conv3x3_args* c) {
 int32_t fyc_conv_small_n(const fyc_conv3x3_args* c, cudaStream_t st) {
   const bool f32out = (c->epilogue & FYC_EPI_OUT_F32) != 0;
   if (c->dtype == FYC_F32) return launch_small_n<float, float>(c, st);
-  if (f32out) return launch_small_n<bf16, float>(c, st);
-  return launch_small_n<bf16, bf16>(c, st);
+  FYC_DISPATCH16(c->dtype, {
+    if (f32out) return launch_small_n<T, float>(c, st);
+    return launch_small_n<T, T>(c, st);
+  })
+  return FYC_OK;
 }

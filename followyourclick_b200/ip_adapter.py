@@ -79,6 +79,13 @@ class IPAttnProcessor(nn.Module):
         self.hidden_size, self.cross_attention_dim, self.scale, self.num_tokens = hidden_size, cross_attention_dim, scale, num_tokens
         self.to_k_ip = nn.Linear(cross_attention_dim or hidden_size, hidden_size, bias=False)
         self.to_v_ip = nn.Linear(cross_attention_dim or hidden_size, hidden_size, bias=False)
+        self._compute_dtype = None          # None: fp32 / bf16 inputs run as they come, anything else in bf16
+
+    def set_compute_dtype(self, dtype):
+        """torch.float32, torch.bfloat16 or torch.float16: the dtype every call runs in, whatever the input's dtype."""
+        ops.check_compute_dtype(dtype)
+        self._compute_dtype = dtype
+        return self
 
     @torch.no_grad()
     def __call__(self, attn, hidden_states, encoder_hidden_states=None, attention_mask=None, temb=None):
@@ -94,7 +101,7 @@ class IPAttnProcessor(nn.Module):
         if nd == 4:
             b, c, h, wd = x.shape
             x = x.view(b, c, h * wd).transpose(1, 2)
-        dt = x.dtype if x.dtype in (torch.float32, torch.bfloat16) else torch.bfloat16
+        dt = self._compute_dtype or (x.dtype if x.dtype in (torch.float32, torch.bfloat16) else torch.bfloat16)
         x = x.to(dt).contiguous()
         B, Lq, C = x.shape
         heads = attn.heads
@@ -149,6 +156,14 @@ class MyIPAdapter:
         self._clip_dim = clip_embeddings_dim or getattr(getattr(image_encoder, "config", None), "projection_dim", 1024)
         self.clip_image_processor = None
         self.image_proj_model = self.init_proj()
+
+    def set_compute_dtype(self, dtype):
+        """forwards to the UNet and the image projector (see ParamTreeModel.set_compute_dtype)"""
+        ops.check_compute_dtype(dtype)
+        for m in (self.unet, self.image_proj_model, getattr(self.unet, "image_proj_model", None)):
+            if m is not None:
+                m.set_compute_dtype(dtype)
+        return self
 
     def init_proj(self):
         return ImageProjModel(cross_attention_dim=self.unet.config.cross_attention_dim, clip_embeddings_dim=self._clip_dim,

@@ -11,6 +11,8 @@ from collections import OrderedDict
 import torch
 from torch import nn
 
+from . import ops
+
 
 class FrozenDict(OrderedDict):
     """Read-only mapping with attribute access (mirror of diffusers.configuration_utils.FrozenDict)."""
@@ -109,6 +111,15 @@ class ParamTreeModel(nn.Module):
         self._invalidate()
         return self
 
+    def set_compute_dtype(self, dtype):
+        """Select the compute dtype directly: torch.float32 (strict fp32, CUDA cores), torch.bfloat16 (the default tensor-core mode) or
+        torch.float16 (the tensor-core mode in IEEE half: the precision of the reference's torch.autocast("cuda"); activations must stay
+        below 65504).  `.to(torch.float16)` / `.half()` keep selecting bf16; this is the one way to run in fp16."""
+        ops.check_compute_dtype(dtype)
+        self._compute_dtype = dtype
+        self._invalidate()
+        return self
+
     def cuda(self, device=None):
         super().cuda(device)
         self._invalidate()
@@ -174,8 +185,8 @@ class ParamTreeModel(nn.Module):
         return self._cached(("c", key), lambda: self._p(key).detach().permute(0, 2, 3, 1).to(self._compute_dtype).contiguous())
 
     def _conv_w_up2(self, key):
-        """phase-summed filter of an upsampler conv, [4, Cout, 2, 2, Cin] (bf16 tensor-core mode only, else None)"""
-        if self._compute_dtype != torch.bfloat16:
+        """phase-summed filter of an upsampler conv, [4, Cout, 2, 2, Cin] (16-bit tensor-core mode only, else None)"""
+        if self._compute_dtype not in (torch.bfloat16, torch.float16):
             return None
         return self._cached(("up2", key), lambda: upsample_phase_weights(self._p(key).detach().float()).to(self._compute_dtype).contiguous())
 

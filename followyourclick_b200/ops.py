@@ -2,7 +2,7 @@
 
 PyTorch is used for device memory (caching allocator), streams and nothing else: every FLOP below is executed by
 a kernel of libfyc_sm90a.so.  All tensors must be CUDA, contiguous in the last dimension; activations are either
-all fp32 (strict parity mode) or all bf16 (tensor-core mode).
+all fp32 (strict parity mode) or all bf16 / all fp16 (tensor-core mode).
 """
 import ctypes as C
 import os
@@ -99,8 +99,18 @@ def _f32vec(t, name):
         raise L.FycError(f"{name}: expected a contiguous fp32 tensor")
 
 
+HALF_DTYPES = (torch.bfloat16, torch.float16)     # the 16-bit storage formats of the tensor-core mode
+COMPUTE_DTYPES = (torch.float32,) + HALF_DTYPES    # what set_compute_dtype accepts
+
+
+def check_compute_dtype(dtype):
+    """the argument check every set_compute_dtype shares: ValueError unless dtype is fp32, bf16 or fp16"""
+    if dtype not in COMPUTE_DTYPES:
+        raise ValueError(f"unsupported compute dtype {dtype}: expected torch.float32, torch.bfloat16 or torch.float16")
+
+
 def tc_ok(dtype, M):
-    return _impl != L.IMPL_SIMT and dtype == torch.bfloat16 and M >= 64 and lib().fyc_tcgen05_available() == 1
+    return _impl != L.IMPL_SIMT and dtype in HALF_DTYPES and M >= 64 and lib().fyc_tcgen05_available() == 1
 
 
 use_ln_fold = os.environ.get("FYC_LN_FOLD", "1") != "0"          # A/B switch: LayerNorm folded into the consuming GEMM's epilogue
@@ -125,16 +135,22 @@ def layernorm_stats(x, eps=1e-5):
     return rstd
 
 
-def _balance_rows_bf16(w, iters=12):
-    """w: fp32 tensor holding bf16-representable values [N, K] -> the same with a handful of elements per row moved by ONE bf16 ulp so
-    that every row sums to ~0 (<= a few 1e-6 instead of ~sqrt(K) * 2^-10 * |w|).  Each step picks, per row, the element whose ulp is
-    closest to the remaining row sum and steps it against the sum's sign; a one-ulp step of a bf16 value is always representable."""
+# significand bits after the point and the smallest normal exponent of each 16-bit format
+_ULP_BITS = {torch.bfloat16: (7, -126), torch.float16: (10, -14)}
+
+
+def _balance_rows(w, dtype, iters=12):
+    """w: fp32 tensor holding `dtype`-representable values [N, K] (dtype bf16 or fp16) -> the same with a handful of elements per row moved
+    by ONE ulp of `dtype` so that every row sums to ~0 (<= a few 1e-6 instead of ~sqrt(K) * ulp * |w|).  Each step picks, per row, the
+    element whose ulp is closest to the remaining row sum and steps it against the sum's sign; a one-ulp step of a representable value is
+    always representable (below the smallest normal exponent the ulp is the subnormal spacing)."""
+    frac, emin = _ULP_BITS[dtype]
     w = w.clone()
     rows = torch.arange(w.shape[0], device=w.device)
     inf = torch.tensor(float("inf"), device=w.device)
     for _ in range(iters):
         r = w.sum(dim=1)
-        ulp = torch.exp2(torch.floor(torch.log2(w.abs().clamp_min(1e-30))) - 7)
+        ulp = torch.exp2(torch.floor(torch.log2(w.abs().clamp_min(1e-30))).clamp_min(emin) - frac)
         ulp = torch.where(w == 0, inf, ulp)
         target = r.abs()[:, None]
         score = torch.where(ulp <= 1.5 * target, (target - ulp).abs(), inf)
@@ -147,13 +163,13 @@ def _balance_rows_bf16(w, iters=12):
 
 def ln_fold_weight(w, gamma, dtype):
     """[N, K] fp32 weight, [K] LayerNorm gain -> the LN-folded GEMM operand: gamma-scaled, every row centred (the mean of LN's input then
-    cancels inside the product: x W"^T = x W'^T - mean colsum), rounded ONCE to the compute dtype; in bf16 the rounded rows are
-    re-balanced to sum to zero (_balance_rows_bf16): the leftover row sum is what a large row mean would multiply - with it the fold is
+    cancels inside the product: x W"^T = x W'^T - mean colsum), rounded ONCE to the compute dtype; in bf16 / fp16 the rounded rows are
+    re-balanced to sum to zero (_balance_rows): the leftover row sum is what a large row mean would multiply - with it the fold is
     as accurate as LN -> bf16 -> GEMM for row means of 100 sigma, without it only for means below ~2 sigma (tests/test_kernels_gpu.py)."""
     wp = w.float() * gamma.float()[None, :]
     wc = (wp - wp.mean(dim=1, keepdim=True)).to(dtype)
-    if dtype == torch.bfloat16:
-        wc = _balance_rows_bf16(wc.float()).to(dtype)
+    if dtype in HALF_DTYPES:
+        wc = _balance_rows(wc.float(), dtype).to(dtype)
     return wc.contiguous()
 
 
@@ -286,7 +302,7 @@ def groupnorm(x, gamma, beta, groups, eps, silu=False, stat_batches=None, x2=Non
     _cuda(x, "groupnorm.x"); _f32vec(gamma, "groupnorm.gamma"); _f32vec(beta, "groupnorm.beta"); _cuda(x2, "groupnorm.x2")
     assert x.is_contiguous()
     C1 = x.shape[-1]
-    vec = 8 if x.dtype == torch.bfloat16 else 4
+    vec = 8 if x.dtype in HALF_DTYPES else 4
     if x2 is not None and not (use_dual_source and C1 % vec == 0 and x2.shape[-1] % vec == 0):
         x, x2 = concat_channels(x, x2.contiguous()), None
         C1 = x.shape[-1]
@@ -351,8 +367,8 @@ def attention(q, k, v, heads, scale, out=None, out_alpha=1.0, accumulate=False, 
 
 
 def transpose_tokens(x, col0, C):
-    """x [NB, L, ld] (bf16) -> columns [col0, col0+C) transposed per batch entry: [NB, C, L]."""
-    assert x.dtype == torch.bfloat16 and x.dim() == 3 and x.stride(2) == 1 and x.stride(0) == x.shape[1] * x.stride(1)
+    """x [NB, L, ld] (bf16 / fp16) -> columns [col0, col0+C) transposed per batch entry: [NB, C, L]."""
+    assert x.dtype in HALF_DTYPES and x.dim() == 3 and x.stride(2) == 1 and x.stride(0) == x.shape[1] * x.stride(1)
     NB, L, _ = x.shape
     out = torch.empty((NB, C, L), dtype=x.dtype, device=x.device)
     with _rec("transpose", 0, 2 * NB * L * C * 2):
@@ -360,8 +376,15 @@ def transpose_tokens(x, col0, C):
     return out
 
 
+def _tc_entry(name, t):
+    """the wgmma attention entry point for t's 16-bit dtype: `name` (bf16) or `name`_f16 (fp16)"""
+    if t.dtype not in HALF_DTYPES:
+        raise L.FycError(f"{name}: 16-bit operands required (got {t.dtype})")
+    return getattr(lib(), name + "_f16" if t.dtype == torch.float16 else name)
+
+
 def self_attention_tc_ok(dtype, L, D):
-    return _impl != L_SIMT and dtype == torch.bfloat16 and D in (40, 64) and L % 128 == 0 and lib().fyc_tcgen05_available() == 1
+    return _impl != L_SIMT and dtype in HALF_DTYPES and D in (40, 64) and L % 128 == 0 and lib().fyc_tcgen05_available() == 1
 
 
 def self_attention_tc(qk, q_col0, k_col0, vt, heads, D, scale):
@@ -370,7 +393,7 @@ def self_attention_tc(qk, q_col0, k_col0, vt, heads, D, scale):
     NB, L, _ = qk.shape
     out = torch.empty((NB, L, heads * D), dtype=qk.dtype, device=qk.device)
     with _rec("attention_tc", 4.0 * NB * heads * L * L * D, qk.element_size() * (4 * NB * L * heads * D)):
-        check(lib().fyc_self_attention_tc(ptr(qk), qk.stride(1), q_col0, k_col0, ptr(vt), ptr(out), out.stride(1), NB, heads, L, D,
+        check(_tc_entry("fyc_self_attention_tc", qk)(ptr(qk), qk.stride(1), q_col0, k_col0, ptr(vt), ptr(out), out.stride(1), NB, heads, L, D,
                                           float(scale), stream_ptr()))
     return out
 
@@ -379,7 +402,7 @@ use_attn_d80 = os.environ.get("FYC_ATTN_D80", "1") != "0"        # A/B switch: h
 
 
 def self_attention_tc80_ok(dtype, L, D):
-    return use_attn_d80 and _impl != L_SIMT and dtype == torch.bfloat16 and D == 80 and L % 256 == 0 and lib().fyc_tcgen05_available() == 1
+    return use_attn_d80 and _impl != L_SIMT and dtype in HALF_DTYPES and D == 80 and L % 256 == 0 and lib().fyc_tcgen05_available() == 1
 
 
 def self_attention_tc_d80(qkv, q_col0, k_col0, vt, heads, scale):
@@ -389,7 +412,7 @@ def self_attention_tc_d80(qkv, q_col0, k_col0, vt, heads, scale):
     D = 80
     out = torch.empty((NB, L, heads * D), dtype=qkv.dtype, device=qkv.device)
     with _rec(f"attention_tc80[{NB}x{heads}x{L}]" if _prof_shapes else "attention_tc", 4.0 * NB * heads * L * L * D, qkv.element_size() * (4 * NB * L * heads * D)):
-        check(lib().fyc_self_attention_tc_d80(ptr(qkv), qkv.stride(1), q_col0, k_col0, ptr(vt), ptr(out), out.stride(1), NB, heads, L,
+        check(_tc_entry("fyc_self_attention_tc_d80", qkv)(ptr(qkv), qkv.stride(1), q_col0, k_col0, ptr(vt), ptr(out), out.stride(1), NB, heads, L,
                                               float(scale), stream_ptr()))
     return out
 
@@ -399,7 +422,7 @@ CROSS_LK, CROSS_LK2 = 80, 16                                      # padded key c
 
 
 def cross_attention_tc_ok(dtype, D, Lk, Lk2):
-    return (use_cross_tc and _impl != L_SIMT and dtype == torch.bfloat16 and D in (40, 64, 80) and 1 <= Lk <= CROSS_LK and 0 <= Lk2 <= CROSS_LK2
+    return (use_cross_tc and _impl != L_SIMT and dtype in HALF_DTYPES and D in (40, 64, 80) and 1 <= Lk <= CROSS_LK and 0 <= Lk2 <= CROSS_LK2
             and lib().fyc_tcgen05_available() == 1)
 
 
@@ -420,7 +443,7 @@ def cross_attention_tc(q, k, vt, heads, D, scale, Lk, out, k2=None, vt2=None, Lk
     assert q.stride(0) == Lq * q.stride(1) and out.stride(0) == Lq * out.stride(1) and k.shape[0] * kv_batch_div == NB
     with _rec(f"cross_attention_tc[{NB}x{heads}x{Lq}x{Lk}+{Lk2}x{D}]" if _prof_shapes else "cross_attention_tc", 4.0 * NB * heads * Lq * (Lk + Lk2) * D,
               q.element_size() * 2 * NB * Lq * heads * D):
-        check(lib().fyc_cross_attention_tc(ptr(q), q.stride(1), 0, ptr(k), k.stride(1), ptr(vt), ptr(k2), k2.stride(1) if k2 is not None else 0,
+        check(_tc_entry("fyc_cross_attention_tc", q)(ptr(q), q.stride(1), 0, ptr(k), k.stride(1), ptr(vt), ptr(k2), k2.stride(1) if k2 is not None else 0,
                                            ptr(vt2), ptr(out), out.stride(1), NB, heads, Lq, D, Lk, Lk2, kv_batch_div, float(scale), float(out_alpha),
                                            float(alpha2), stream_ptr()))
     return out

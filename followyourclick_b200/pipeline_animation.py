@@ -157,6 +157,15 @@ class AnimationPipeline:
                 m.to(device) if dtype is None else m.to(device, dtype)
         return self
 
+    def set_compute_dtype(self, dtype):
+        """Run the engine's models (UNet, VAE, IP-Adapter) in `dtype`: torch.float32, torch.bfloat16 or torch.float16
+        (ParamTreeModel.set_compute_dtype).  The text / image encoders are not engine models and keep their own dtype."""
+        ops.check_compute_dtype(dtype)
+        for m in (self.unet, self.vae, self.ip_adapter):
+            if m is not None:
+                m.set_compute_dtype(dtype)
+        return self
+
     @property
     def device(self):
         return self.unet.device

@@ -2,7 +2,7 @@
 
 Same constructor kwargs, same state-dict keys (SURVEY App. E), same ``forward`` signature and ``.sample`` output as
 the reference class, so ``scripts/inference.py`` and ``AnimationPipeline`` can use it unchanged.  The forward pass is
-not an nn.Module graph: activations live as channels-last tokens ``[B*F, H, W, C]`` in bf16 (tensor-core mode) or
+not an nn.Module graph: activations live as channels-last tokens ``[B*F, H, W, C]`` in bf16 or fp16 (tensor-core mode) or
 fp32 (strict mode) and every operator is a libfyc_sm90a kernel (followyourclick_b200.ops):
 
   ResnetBlock3D  (resnet.py:296-342)   GN(cross-frame)+SiLU -> conv3x3 [+bias +time-emb row bias] -> GN+SiLU ->
@@ -241,7 +241,7 @@ class UNet3DConditionModel(ParamTreeModel):
         # upcast_attention (SD-2.x) makes the reference form Q K^T and the softmax in fp32 (diffusers/models/attention.py:649-660).  Every
         # engine attention kernel already does, whatever the storage dtype: the wgmma kernels (attention_tc.cu) and the mma.sync kernel
         # (attention_mma.cu) accumulate S in fp32 registers and run the softmax on them, the SIMT kernel (attention_simt.cu) and the
-        # temporal kernels (temporal_mma.cu, attention_simt.cu) likewise; bf16 is only the operand and output format.  So the flag
+        # temporal kernels (temporal_mma.cu, attention_simt.cu) likewise; bf16 / fp16 is only the operand and output format.  So the flag
         # changes nothing here and is accepted as is.
         unsupported = dict(center_input_sample=False, only_cross_attention=False, dual_cross_attention=False,
                            class_embed_type=None, num_class_embeds=None, resnet_time_scale_shift="default", use_pseudo_conv3d=False,
@@ -665,7 +665,7 @@ class UNet3DConditionModel(ParamTreeModel):
         conv runs on the tensor cores, else the model's true input channels."""
         w = self._p("conv_in.weight")
         cin = w.shape[1]
-        if self._compute_dtype == torch.bfloat16 and cin % 8 != 0 and cin <= 16 and ops.tc_ok(torch.bfloat16, 1 << 20):
+        if self._compute_dtype in ops.HALF_DTYPES and cin % 8 != 0 and cin <= 16 and ops.tc_ok(self._compute_dtype, 1 << 20):
             return 16
         return cin
 

@@ -11,7 +11,8 @@
  *     never synchronises, never touches the default stream: all work is enqueued on `stream`;
  *   - return value 0 = OK, non-zero = error, message via fyc_last_error() (thread-local);
  *   - activations are channels-last "tokens": [images(B*F), H*W, C] contiguous unless a leading dimension
- *     is passed; `dtype` selects the storage type of activations/weights (accumulation is always fp32);
+ *     is passed; `dtype` selects the storage type of activations/weights (accumulation is always fp32); "16-bit" below means
+ *     FYC_BF16 or FYC_F16;
  *   - small per-channel vectors (bias, norm gamma/beta) are always fp32.
  */
 #ifndef FYC_H_
@@ -27,7 +28,9 @@ extern "C" {
 #define FYC_VERSION 100 /* 0.1.0 */
 
 enum { FYC_OK = 0, FYC_ERR_INVALID = 1, FYC_ERR_CUDA = 2, FYC_ERR_UNSUPPORTED = 3 };
-enum { FYC_F32 = 0, FYC_BF16 = 1 };
+/* storage dtypes.  FYC_F16 (IEEE half) is accepted wherever FYC_BF16 is, with the same layouts and eligibility rules: its 11
+ * significand bits round about 8x finer than bf16's 8, and its range ends at 65504 (the caller keeps activations within it). */
+enum { FYC_F32 = 0, FYC_BF16 = 1, FYC_F16 = 2 };
 /* GEMM / conv implementation selector */
 enum { FYC_IMPL_AUTO = 0, FYC_IMPL_SIMT = 1, FYC_IMPL_TCGEN05 = 2 };
 /* epilogue flags */
@@ -100,7 +103,7 @@ typedef struct {
                                    right only - diffusers Downsample2D with padding=0, F.pad(x, (0,1,0,1)) + valid conv
                                    (diffusers/models/resnet.py:183-188), the VAE Encoder's downsamplers (vae.py:95);
                                    Ho = H/2 either way, input row = 2*oh + kh instead of 2*oh + kh - 1 */
-  const void* w_phases;         /* optional (upsample == 2, bf16): the filter pre-summed per output parity, [4 phases = 2*py+px]
+  const void* w_phases;         /* optional (upsample == 2, 16-bit): the filter pre-summed per output parity, [4 phases = 2*py+px]
                                    [Cout][2][2][Cin].  nearest-x2 followed by a padded 3x3 conv is, for each output parity (py, px),
                                    a 2x2 conv on the LOW-resolution image: rows {oh-1 | w[0], oh | w[1]+w[2]} for py = 0 and
                                    {oh | w[0]+w[1], oh+1 | w[2]} for py = 1 (columns alike) - 16 instead of 36 MACs per input
@@ -140,7 +143,7 @@ int32_t fyc_layernorm(const void* x, const float* gamma, const float* beta, void
                       void* stream);
 
 /* LayerNorm statistics only (biased variance + eps like nn.LayerNorm) for a GEMM launched with FYC_EPI_LNFOLD: rstd[m] (fp32).  `aug` is
- * optional (NULL: not written): [m][8] bf16 = [m_hi, m_hi, m_lo, m_lo, 0, 0, 0, 0] with mean_m = m_hi + m_lo, for callers that want the
+ * optional (NULL: not written): [m][8] in `dtype` (bf16 for fp32 rows) = [m_hi, m_hi, m_lo, m_lo, 0, 0, 0, 0] with mean_m = m_hi + m_lo, for callers that want the
  * row mean as a second K segment of a GEMM (fyc_gemm_args.A2) instead of centred weights. */
 int32_t fyc_layernorm_stats(const void* x, float* rstd, void* aug, int64_t M, int64_t C, float eps, int32_t dtype, void* stream);
 
@@ -181,12 +184,18 @@ int32_t fyc_temporal_attention(const void* qkv, void* out, int64_t B, int64_t F,
  * (V transposed per image, fyc_transpose_tokens); out: [NB, L, ldo], head h at columns [h*D, (h+1)*D). */
 int32_t fyc_self_attention_tc(const void* qk, int64_t ldqk, int64_t q_col0, int64_t k_col0, const void* vt, void* out,
                               int64_t ldo, int64_t NB, int64_t heads, int64_t L, int64_t D, float scale, void* stream);
+/* The same with fp16 operands and output (FYC_F16 storage). */
+int32_t fyc_self_attention_tc_f16(const void* qk, int64_t ldqk, int64_t q_col0, int64_t k_col0, const void* vt, void* out,
+                                  int64_t ldo, int64_t NB, int64_t heads, int64_t L, int64_t D, float scale, void* stream);
 /* The same for head dim 80, L % 256 == 0 - the level-1 attn1 (1024 tokens at cfg2, 2304 at cfg5).  qkv: [NB, L, ldqkv] bf16, the fused
  * [q | k | v] projection UNPADDED: q head h at columns [q_col0 + 80 h, +80), k at [k_col0 + 80 h, +80); each head's second 64-column
  * TMA atom overlaps the next head, whose columns are never multiplied (QK^T issues 5 k-steps of 16), so the row only has to extend 48
  * columns past the last k head (the v block does).  vt: [NB, heads * 80, L]; out: [NB, L, ldo]. */
 int32_t fyc_self_attention_tc_d80(const void* qkv, int64_t ldqkv, int64_t q_col0, int64_t k_col0, const void* vt, void* out,
                                   int64_t ldo, int64_t NB, int64_t heads, int64_t L, float scale, void* stream);
+/* The same with fp16 operands and output. */
+int32_t fyc_self_attention_tc_d80_f16(const void* qkv, int64_t ldqkv, int64_t q_col0, int64_t k_col0, const void* vt, void* out,
+                                      int64_t ldo, int64_t NB, int64_t heads, int64_t L, float scale, void* stream);
 /* Cross-attention against a SHORT, step-invariant context on the tensor cores (head dim 40, 64 or 80; bf16): attn2 of every transformer block
  * (diffusers/models/attention.py:649-678) and, with the second context, the whole IP-Adapter cross-attention in one launch
  * (animatediff/models/attention.py:92-120, ip_adapter/attention_processor.py:137-168):
@@ -202,7 +211,11 @@ int32_t fyc_self_attention_tc_d80(const void* qkv, int64_t ldqkv, int64_t q_col0
 int32_t fyc_cross_attention_tc(const void* q, int64_t ldq, int64_t q_col0, const void* k, int64_t ldk, const void* vt, const void* k2,
                                int64_t ldk2, const void* vt2, void* out, int64_t ldo, int64_t NB, int64_t heads, int64_t Lq, int64_t D,
                                int64_t Lk, int64_t Lk2, int64_t kv_batch_div, float scale, float out_alpha, float alpha2, void* stream);
-/* in [NB, L, ld] columns [col0, col0 + C) (bf16) -> out [NB, C, L] */
+/* The same with fp16 operands and output. */
+int32_t fyc_cross_attention_tc_f16(const void* q, int64_t ldq, int64_t q_col0, const void* k, int64_t ldk, const void* vt, const void* k2,
+                                   int64_t ldk2, const void* vt2, void* out, int64_t ldo, int64_t NB, int64_t heads, int64_t Lq, int64_t D,
+                                   int64_t Lk, int64_t Lk2, int64_t kv_batch_div, float scale, float out_alpha, float alpha2, void* stream);
+/* in [NB, L, ld] columns [col0, col0 + C) (any 16-bit type: the values are moved, not converted) -> out [NB, C, L] */
 int32_t fyc_transpose_tokens(const void* in, void* out, int64_t NB, int64_t L, int64_t C, int64_t ld, int64_t col0,
                              void* stream);
 /* Row softmax of fp32 scores (VAE AttentionBlock, diffusers/models/attention.py:366), output in `dtype`. */
