@@ -20,10 +20,9 @@
 // tiles (double-buffered Q).  Per tile: S_t = Q K_t^T (N = 80) and S_i = Q K_i^T (N = 16) -> two INDEPENDENT softmaxes, normalised
 // in registers (the whole context is one tile: no online rescaling) and pre-scaled by out_alpha / l_t and alpha2 / l_i -> P_t, P_i
 // (bf16 registers) -> O = P_t V_t + P_i V_i in ONE accumulator -> bf16 out, written once.  Padding keys are masked to -inf.
-#include <cuda.h>
 #include <stdlib.h>
 
-#include "common.cuh"
+#include "tma.cuh"
 #include "wgmma.cuh"
 
 namespace {
@@ -32,41 +31,6 @@ constexpr int BQ = 128, BKV = 128;
 constexpr int ATOM_BYTES = BQ * 128;                            // 16 KB: 128 rows x 64 bf16 columns
 constexpr int NTHREADS = 256;                                   // two warpgroups
 
-__device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
-  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count));
-}
-__device__ __forceinline__ void mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
-  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "WAIT_LOOP:\n\t"
-      "mbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n\t"
-      "@p bra.uni WAIT_DONE;\n\t"
-      "bra.uni WAIT_LOOP;\n\t"
-      "WAIT_DONE:\n\t"
-      "}" ::"r"(smem_u32(bar)), "r"(parity) : "memory");
-}
-__device__ __forceinline__ void tma_load_3d(const CUtensorMap* map, uint64_t* bar, void* dst, int c0, int c1, int c2) {
-  asm volatile(
-      "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];"
-      ::"r"(smem_u32(dst)), "l"(reinterpret_cast<uint64_t>(map)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2)
-      : "memory");
-}
-__device__ __forceinline__ void tma_load_4d(const CUtensorMap* map, uint64_t* bar, void* dst, int c0, int c1, int c2, int c3) {
-  asm volatile(
-      "cp.async.bulk.tensor.4d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], [%2];"
-      ::"r"(smem_u32(dst)), "l"(reinterpret_cast<uint64_t>(map)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
-      : "memory");
-}
-__device__ __forceinline__ float ex2(float x) {
-  float y;
-  asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
-  return y;
-}
 __device__ __forceinline__ float quad_max(float v) {
   v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, 1));
   return fmaxf(v, __shfl_xor_sync(0xffffffffu, v, 2));
@@ -113,7 +77,7 @@ attention_tc_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_cons
   constexpr int K_BYTES = KA * ATOM_BYTES, V_BYTES = 2 * VBOX;
   constexpr int OFF_K = KA * ATOM_BYTES, OFF_V = OFF_K + 2 * K_BYTES, OFF_BAR = OFF_V + 2 * V_BYTES;
   extern __shared__ __align__(1024) uint8_t smem_raw[];
-  uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
+  uint8_t* smem = smem_raw + pad1024(smem_raw);
   uint64_t* qbar = reinterpret_cast<uint64_t*>(smem + OFF_BAR);
   uint64_t* full = qbar + 1;                       // [2]
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, wg = warp >> 2, q = lane & 3;
@@ -130,7 +94,7 @@ attention_tc_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_cons
   };
   if (threadIdx.x == 0) {
     mbar_init(qbar, 1); mbar_init(&full[0], 1); mbar_init(&full[1], 1);
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    mbar_init_fence();
     mbar_expect_tx(qbar, KA * ATOM_BYTES);
 #pragma unroll
     for (int a = 0; a < KA; ++a) tma_load_4d(&map_q, qbar, smem + a * ATOM_BYTES, 64 * a, q0, h, n);
@@ -166,14 +130,14 @@ attention_tc_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_cons
       mx1 = fmaxf(mx1, fmaxf(sc[4 * t + 2], sc[4 * t + 3]));
     }
     const float mn0 = fmaxf(m0, quad_max(mx0)), mn1 = fmaxf(m1, quad_max(mx1));   // running maxima of the RAW scores (scale > 0)
-    const float c0 = ex2((m0 - mn0) * sl2), c1 = ex2((m1 - mn1) * sl2);
+    const float c0 = ex2_approx((m0 - mn0) * sl2), c1 = ex2_approx((m1 - mn1) * sl2);
     m0 = mn0; m1 = mn1;
     const float nb0 = -mn0 * sl2, nb1 = -mn1 * sl2;
     float rs0 = 0.f, rs1 = 0.f;
 #pragma unroll
     for (int t = 0; t < BKV / 8; ++t) {
-      sc[4 * t] = ex2(fmaf(sc[4 * t], sl2, nb0)); sc[4 * t + 1] = ex2(fmaf(sc[4 * t + 1], sl2, nb0));
-      sc[4 * t + 2] = ex2(fmaf(sc[4 * t + 2], sl2, nb1)); sc[4 * t + 3] = ex2(fmaf(sc[4 * t + 3], sl2, nb1));
+      sc[4 * t] = ex2_approx(fmaf(sc[4 * t], sl2, nb0)); sc[4 * t + 1] = ex2_approx(fmaf(sc[4 * t + 1], sl2, nb0));
+      sc[4 * t + 2] = ex2_approx(fmaf(sc[4 * t + 2], sl2, nb1)); sc[4 * t + 3] = ex2_approx(fmaf(sc[4 * t + 3], sl2, nb1));
       rs0 += sc[4 * t] + sc[4 * t + 1]; rs1 += sc[4 * t + 2] + sc[4 * t + 3];
     }
     l0 = l0 * c0 + rs0; l1 = l1 * c1 + rs1;
@@ -221,8 +185,8 @@ __device__ __forceinline__ void softmax_ctx(float* sc, int Lk, float wgt, float 
   float rs0 = 0.f, rs1 = 0.f;
 #pragma unroll
   for (int t = 0; t < NT; ++t) {
-    sc[4 * t] = ex2(fmaf(sc[4 * t], sl2, nb0)); sc[4 * t + 1] = ex2(fmaf(sc[4 * t + 1], sl2, nb0));
-    sc[4 * t + 2] = ex2(fmaf(sc[4 * t + 2], sl2, nb1)); sc[4 * t + 3] = ex2(fmaf(sc[4 * t + 3], sl2, nb1));
+    sc[4 * t] = ex2_approx(fmaf(sc[4 * t], sl2, nb0)); sc[4 * t + 1] = ex2_approx(fmaf(sc[4 * t + 1], sl2, nb0));
+    sc[4 * t + 2] = ex2_approx(fmaf(sc[4 * t + 2], sl2, nb1)); sc[4 * t + 3] = ex2_approx(fmaf(sc[4 * t + 3], sl2, nb1));
     rs0 += sc[4 * t] + sc[4 * t + 1]; rs1 += sc[4 * t + 2] + sc[4 * t + 3];
   }
   const float f0 = wgt / quad_sum(rs0), f1 = wgt / quad_sum(rs1);
@@ -240,7 +204,7 @@ attention_cx_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_cons
   constexpr int OFF_KT = 2 * Q_BYTES, OFF_VT = OFF_KT + KA * KT_ATOM, OFF_KI = OFF_VT + 2 * VBOX, OFF_VI = OFF_KI + KA * KI_ATOM;
   constexpr int OFF_BAR = OFF_VI + VBOX;
   extern __shared__ __align__(1024) uint8_t smem_raw[];
-  uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
+  uint8_t* smem = smem_raw + pad1024(smem_raw);
   uint64_t* cbar = reinterpret_cast<uint64_t*>(smem + OFF_BAR);
   uint64_t* qfull = cbar + 1;                      // [2]
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, wg = warp >> 2, q = lane & 3;
@@ -255,7 +219,7 @@ attention_cx_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_cons
   };
   if (threadIdx.x == 0) {
     mbar_init(cbar, 1); mbar_init(&qfull[0], 1); mbar_init(&qfull[1], 1);
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    mbar_init_fence();
     const int dkp = KA == 1 ? 64 : D;
     mbar_expect_tx(cbar, KA * KT_ATOM + 2 * VBOX + (two ? KA * KI_ATOM + VBOX : 0));
 #pragma unroll
@@ -342,35 +306,6 @@ __global__ void __launch_bounds__(256) transpose_tokens_kernel(const bf16* __res
   }
 }
 
-typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
-                                  const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
-                                  CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-EncodeTiledFn encode_fn() {
-  static EncodeTiledFn fn = nullptr;
-  static bool tried = false;
-  if (!tried) {
-    tried = true;
-    void* ptr = nullptr;
-    cudaDriverEntryPointQueryResult q;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &ptr, cudaEnableDefault, &q) == cudaSuccess && q == cudaDriverEntryPointSuccess)
-      fn = reinterpret_cast<EncodeTiledFn>(ptr);
-    else
-      (void)cudaGetLastError();
-  }
-  return fn;
-}
-int32_t make_map(CUtensorMap* m, const void* base, int rank, const uint64_t* dims, const uint64_t* strides, const uint32_t* box, int32_t dt) {
-  EncodeTiledFn fn = encode_fn();
-  FYC_CHECK(fn != nullptr, "attention(tensor cores): cuTensorMapEncodeTiled unavailable");
-  cuuint64_t gd[5], gs[4]; cuuint32_t bx[5], es[5];
-  for (int i = 0; i < rank; ++i) { gd[i] = dims[i]; bx[i] = box[i]; es[i] = 1; }
-  for (int i = 0; i + 1 < rank; ++i) gs[i] = strides[i];
-  CUresult r = fn(m, dt == FYC_F16 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, (cuuint32_t)rank, const_cast<void*>(base), gd, gs, bx, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                  CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  FYC_CHECK(r == CUDA_SUCCESS, "attention(tensor cores): cuTensorMapEncodeTiled failed (%d)", (int)r);
-  return FYC_OK;
-}
-
 template <int KA, int KS, int DV, int D, typename T>
 int32_t launch_self(const CUtensorMap& mq, const CUtensorMap& mk, const CUtensorMap& mv, const AttnTcParams& p, int64_t NB, cudaStream_t st) {
   constexpr int smem = self_smem<KA, KS, DV, D>();
@@ -420,16 +355,16 @@ static int32_t self_attention_tc(int32_t dt, const void* qk, int64_t ldqk, int64
     uint64_t dims[4] = {64, (uint64_t)L, (uint64_t)heads, (uint64_t)NB};
     uint64_t str[3] = {(uint64_t)ldqk * 2, 128, (uint64_t)L * ldqk * 2};
     uint32_t box[4] = {64, (uint32_t)BQ, 1, 1};
-    int32_t rc = make_map(&mq, (const uint16_t*)qk + q_col0, 4, dims, str, box, dt);
+    int32_t rc = encode_map(&mq, (const uint16_t*)qk + q_col0, 4, dims, str, box, tma_dtype(dt));
     if (rc) return rc;
-    rc = make_map(&mk, (const uint16_t*)qk + k_col0, 4, dims, str, box, dt);
+    rc = encode_map(&mk, (const uint16_t*)qk + k_col0, 4, dims, str, box, tma_dtype(dt));
     if (rc) return rc;
   }
   {
     uint64_t dims[3] = {(uint64_t)L, (uint64_t)(heads * D), (uint64_t)NB};
     uint64_t str[2] = {(uint64_t)L * 2, (uint64_t)L * heads * D * 2};
     uint32_t box[3] = {64, D == 40 ? 48u : 64u, 1};
-    int32_t rc = make_map(&mv, vt, 3, dims, str, box, dt);
+    int32_t rc = encode_map(&mv, vt, 3, dims, str, box, tma_dtype(dt));
     if (rc) return rc;
   }
   AttnTcParams p;
@@ -460,16 +395,16 @@ static int32_t self_attention_tc_d80(int32_t dt, const void* qkv, int64_t ldqkv,
     uint64_t dims[4] = {128, (uint64_t)L, (uint64_t)heads, (uint64_t)NB};
     uint64_t str[3] = {(uint64_t)ldqkv * 2, (uint64_t)D * 2, (uint64_t)L * ldqkv * 2};
     uint32_t box[4] = {64, (uint32_t)BQ, 1, 1};
-    int32_t rc = make_map(&mq, (const uint16_t*)qkv + q_col0, 4, dims, str, box, dt);
+    int32_t rc = encode_map(&mq, (const uint16_t*)qkv + q_col0, 4, dims, str, box, tma_dtype(dt));
     if (rc) return rc;
-    rc = make_map(&mk, (const uint16_t*)qkv + k_col0, 4, dims, str, box, dt);
+    rc = encode_map(&mk, (const uint16_t*)qkv + k_col0, 4, dims, str, box, tma_dtype(dt));
     if (rc) return rc;
   }
   {
     uint64_t dims[3] = {(uint64_t)L, (uint64_t)(heads * D), (uint64_t)NB};
     uint64_t str[2] = {(uint64_t)L * 2, (uint64_t)L * heads * D * 2};
     uint32_t box[3] = {64, (uint32_t)D, 1};
-    int32_t rc = make_map(&mv, vt, 3, dims, str, box, dt);
+    int32_t rc = encode_map(&mv, vt, 3, dims, str, box, tma_dtype(dt));
     if (rc) return rc;
   }
   AttnTcParams p;
@@ -504,19 +439,19 @@ static int32_t cross_attention_tc(int32_t dt, const void* q, int64_t ldq, int64_
     uint64_t dims[3] = {(uint64_t)(heads * D), (uint64_t)Lq, (uint64_t)NB};
     uint64_t str[2] = {(uint64_t)ldq * 2, (uint64_t)Lq * ldq * 2};
     uint32_t box[3] = {64, (uint32_t)BQ, 1};
-    int32_t rc = make_map(&mq, (const uint16_t*)q + q_col0, 3, dims, str, box, dt);
+    int32_t rc = encode_map(&mq, (const uint16_t*)q + q_col0, 3, dims, str, box, tma_dtype(dt));
     if (rc) return rc;
   }
   {
     uint64_t dims[3] = {(uint64_t)(heads * DKP), (uint64_t)CX_LK, (uint64_t)NBc};
     uint64_t str[2] = {(uint64_t)ldk * 2, (uint64_t)CX_LK * ldk * 2};
     uint32_t box[3] = {64, (uint32_t)CX_LK, 1};
-    int32_t rc = make_map(&mk, k, 3, dims, str, box, dt);
+    int32_t rc = encode_map(&mk, k, 3, dims, str, box, tma_dtype(dt));
     if (rc) return rc;
     uint64_t vd[3] = {(uint64_t)CX_LK, (uint64_t)(heads * D), (uint64_t)NBc};
     uint64_t vs[2] = {CX_LK * 2, (uint64_t)(CX_LK * heads * D * 2)};
     uint32_t vb[3] = {64, DV, 1};
-    rc = make_map(&mv, vt, 3, vd, vs, vb, dt);
+    rc = encode_map(&mv, vt, 3, vd, vs, vb, tma_dtype(dt));
     if (rc) return rc;
   }
   mk2 = mk; mv2 = mv;
@@ -524,12 +459,12 @@ static int32_t cross_attention_tc(int32_t dt, const void* q, int64_t ldq, int64_
     uint64_t dims[3] = {(uint64_t)(heads * DKP), (uint64_t)CX_LK2, (uint64_t)NBc};
     uint64_t str[2] = {(uint64_t)ldk2 * 2, (uint64_t)CX_LK2 * ldk2 * 2};
     uint32_t box[3] = {64, (uint32_t)CX_LK2, 1};
-    int32_t rc = make_map(&mk2, k2, 3, dims, str, box, dt);
+    int32_t rc = encode_map(&mk2, k2, 3, dims, str, box, tma_dtype(dt));
     if (rc) return rc;
     uint64_t vd[3] = {(uint64_t)CX_LK2, (uint64_t)(heads * D), (uint64_t)NBc};
     uint64_t vs[2] = {CX_LK2 * 2, (uint64_t)(CX_LK2 * heads * D * 2)};
     uint32_t vb[3] = {64, DV, 1};
-    rc = make_map(&mv2, vt2, 3, vd, vs, vb, dt);
+    rc = encode_map(&mv2, vt2, 3, vd, vs, vb, tma_dtype(dt));
     if (rc) return rc;
   }
   AttnCxParams p;

@@ -145,6 +145,25 @@ template <typename T, int V> __device__ __forceinline__ void store_vec(T* p, con
   else *p = from_f<T>(f[0]);
 }
 
+__device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
+
+// 16-byte cp.async global -> shared; the first form reads src_bytes (0 or 16) and zero-fills the rest
+__device__ __forceinline__ void cp_async16(void* dst, const void* src, int src_bytes) {
+  asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(smem_u32(dst)), "l"(src), "r"(src_bytes) : "memory");
+}
+__device__ __forceinline__ void cp_async16(void* dst, const void* src) {
+  asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(smem_u32(dst)), "l"(src) : "memory");
+}
+__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
+template <int N> __device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory"); }
+
+__device__ __forceinline__ void ldmatrix_x4(uint32_t* r, const void* p) {
+  asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0, %1, %2, %3}, [%4];" : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]) : "r"(smem_u32(p)));
+}
+__device__ __forceinline__ void ldmatrix_x4_trans(uint32_t* r, const void* p) {
+  asm volatile("ldmatrix.sync.aligned.m8n8.x4.trans.shared.b16 {%0, %1, %2, %3}, [%4];" : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]) : "r"(smem_u32(p)));
+}
+
 // mma.sync m16n8k16, fp32 accumulator c += a b with 16-bit operands T (bf16 | f16)
 template <typename T> __device__ __forceinline__ void mma16816(float* c, const uint32_t* a, uint32_t b0, uint32_t b1) {
   if constexpr (std::is_same<T, f16>::value)
@@ -162,6 +181,13 @@ __device__ __forceinline__ float silu_fast(float x) { return __fdividef(x, 1.0f 
 // exact-erf GELU (F.gelu default; diffusers/models/attention.py:815)
 __device__ __forceinline__ float gelu_erf_f(float x) { return 0.5f * x * (1.0f + erff(x * 0.70710678118654752440f)); }
 
+// single MUFU.EX2 (exp2f() adds denormal-range handling: ~4 instructions per element in an issue-bound kernel)
+__device__ __forceinline__ float ex2_approx(float x) {
+  float y;
+  asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
+  return y;
+}
+
 // exact-erf GELU with erf(z) = 1 - 2^q(z), q = degree-5 least-squares fit of log2(erfc(z)) on [0, 4] (|erf error| <= 7.2e-7,
 // |gelu error| <= 1.3e-6 over all x; fit script in DESIGN.md): ONE MUFU.EX2 + 7 FMAs instead of erff()'s ~30 instructions.
 // (A first version with Abramowitz-Stegun 7.1.26 needed rcp + ex2 = two MUFU ops per element and made the GEGLU epilogue
@@ -173,9 +199,7 @@ __device__ __forceinline__ float gelu_erf_fast(float x) {
   q = fmaf(q, z, -0.9184384942054749f);
   q = fmaf(q, z, -1.6278971433639526f);
   q = fmaf(q, z, -2.8457714051910443e-07f);
-  float e;
-  asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(e) : "f"(q));
-  const float erfv = copysignf(1.0f - e, x);
+  const float erfv = copysignf(1.0f - ex2_approx(q), x);
   return 0.5f * x * (1.0f + erfv);
 }
 

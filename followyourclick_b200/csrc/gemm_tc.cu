@@ -16,9 +16,7 @@
 // by (dy, dx); TMA's out-of-bounds zero fill implements the padding halo.  A plain GEMM is the 1-tap special case.
 // Stride-2 convolutions run on a parity-plane split of the input (fyc_space_to_planes), which turns every tap into
 // a unit-stride shifted read of one plane (tap_img selects the plane).
-#include <cuda.h>
-
-#include "common.cuh"
+#include "tma.cuh"
 #include "wgmma.cuh"
 
 namespace {
@@ -68,52 +66,7 @@ struct TcParams {
   int half_dw, half_dh, half_dn;
 };
 
-// ---------------------------------------------------------------------------------------------- PTX wrappers
-__device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-
-__device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
-  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count));
-}
-__device__ __forceinline__ void mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
-  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
-  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "WAIT_LOOP:\n\t"
-      "mbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n\t"
-      "@p bra.uni WAIT_DONE;\n\t"
-      "bra.uni WAIT_LOOP;\n\t"
-      "WAIT_DONE:\n\t"
-      "}" ::"r"(smem_u32(bar)), "r"(parity) : "memory");
-}
-__device__ __forceinline__ void tma_load_4d(const CUtensorMap* map, uint64_t* bar, void* dst, int c0, int c1, int c2, int c3) {
-  asm volatile(
-      "cp.async.bulk.tensor.4d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], [%2];"
-      ::"r"(smem_u32(dst)), "l"(reinterpret_cast<uint64_t>(map)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
-      : "memory");
-}
-__device__ __forceinline__ void tma_load_3d(const CUtensorMap* map, uint64_t* bar, void* dst, int c0, int c1, int c2) {
-  asm volatile(
-      "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];"
-      ::"r"(smem_u32(dst)), "l"(reinterpret_cast<uint64_t>(map)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2)
-      : "memory");
-}
-__device__ __forceinline__ void tma_store_4d(const CUtensorMap* map, const void* src, int c0, int c1, int c2, int c3) {
-  asm volatile("cp.async.bulk.tensor.4d.global.shared::cta.bulk_group [%0, {%2, %3, %4, %5}], [%1];"
-               ::"l"(reinterpret_cast<uint64_t>(map)), "r"(smem_u32(src)), "r"(c0), "r"(c1), "r"(c2), "r"(c3) : "memory");
-}
-__device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
-// the committed stores have finished reading shared memory (their source may be overwritten)
-__device__ __forceinline__ void bulk_wait_read() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
-// the committed stores are complete
-__device__ __forceinline__ void bulk_wait_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
-// generic-proxy writes to shared memory become visible to the TMA (async proxy) reads that follow
-__device__ __forceinline__ void fence_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
+// ---------------------------------------------------------------------------------------------- warpgroup barrier
 // named barrier over one consumer warpgroup (id 0 is __syncthreads)
 __device__ __forceinline__ void warpgroup_sync(int wg) {
   if (wg == 0) asm volatile("bar.sync 1, 128;" ::: "memory");
@@ -213,7 +166,7 @@ __global__ void __launch_bounds__(NUM_THREADS, 1)
 gemm_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_w, const __grid_constant__ CUtensorMap map_a2,
                const __grid_constant__ CUtensorMap map_out, const __grid_constant__ CUtensorMap map_res, const TcParams p) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
-  uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);     // SWIZZLE_128B operands need 1024-byte alignment
+  uint8_t* smem = smem_raw + pad1024(smem_raw);
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + p.ring_bytes + 2 * p.stg_bytes);
   uint64_t* full = bars;                       // [MAX_STAGES]
   uint64_t* empty = bars + MAX_STAGES;         // [MAX_STAGES]
@@ -234,7 +187,7 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
     for (int s = 0; s < MAX_STAGES; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 256); }   // empty: one arrival per consumer thread
     mbar_init(wbar, 1);
     mbar_init(&rbar[0], 1); mbar_init(&rbar[1], 1);
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    mbar_init_fence();
   }
   __syncthreads();
 
@@ -359,45 +312,6 @@ __global__ void space_to_planes_kernel(const bf16* __restrict__ x, bf16* __restr
 }
 
 // ---------------------------------------------------------------------------------------------- host side
-typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
-                                  const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
-                                  CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-
-EncodeTiledFn get_encode_fn() {
-  static EncodeTiledFn fn = nullptr;
-  static bool tried = false;
-  if (!tried) {
-    tried = true;
-    void* ptr = nullptr;
-    cudaDriverEntryPointQueryResult qres;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &ptr, cudaEnableDefault, &qres) == cudaSuccess &&
-        qres == cudaDriverEntryPointSuccess)
-      fn = reinterpret_cast<EncodeTiledFn>(ptr);
-    else
-      (void)cudaGetLastError();
-  }
-  return fn;
-}
-
-// TMA element type of a 16-bit storage dtype (FYC_BF16 | FYC_F16)
-CUtensorMapDataType map_dtype(int32_t dt) { return dt == FYC_F16 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16; }
-
-int32_t encode_map(CUtensorMap* m, const void* base, int rank, const uint64_t* dims, const uint64_t* strides_bytes,
-                   const uint32_t* box, CUtensorMapDataType dtype, CUtensorMapSwizzle swizzle = CU_TENSOR_MAP_SWIZZLE_128B) {
-  EncodeTiledFn fn = get_encode_fn();
-  FYC_CHECK(fn != nullptr, "tensor-core path: cuTensorMapEncodeTiled driver entry point unavailable");
-  cuuint64_t gdim[5]; cuuint64_t gstr[4]; cuuint32_t bx[5]; cuuint32_t es[5];
-  for (int i = 0; i < rank; ++i) { gdim[i] = dims[i]; bx[i] = box[i]; es[i] = 1; }
-  for (int i = 0; i + 1 < rank; ++i) gstr[i] = strides_bytes[i];
-  CUresult r = fn(m, dtype, (cuuint32_t)rank, const_cast<void*>(base), gdim, gstr, bx, es,
-                  CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
-                  CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  FYC_CHECK(r == CUDA_SUCCESS, "cuTensorMapEncodeTiled failed with CUresult %d (rank %d dims %llu %llu %llu %llu)", (int)r, rank,
-            (unsigned long long)dims[0], (unsigned long long)dims[1], (unsigned long long)(rank > 2 ? dims[2] : 0),
-            (unsigned long long)(rank > 3 ? dims[3] : 0));
-  return FYC_OK;
-}
-
 // Output (or residual) map of a launch: `cols` channels by W x H x NB pixels at `base`, pixel (w, h, n) at element offset
 // w * sw + h * sh + n * sn.  The dimensions are the tensor's true extent, so TMA clips the rows past M and the columns past N_out.
 // Box: one 32-byte column box of a warpgroup's half patch (choose_tiles sets the split).
@@ -409,7 +323,7 @@ int32_t encode_out_map(CUtensorMap* m, const void* base, const TcParams& p, int3
   uint64_t str[3] = {sw * es, sh * es, sn * es};
   uint32_t box[4] = {(uint32_t)(OUT_BOX_BYTES / es), (uint32_t)(p.half_dw ? p.half_dw : p.bw), (uint32_t)(p.half_dh ? p.half_dh : p.bh),
                      (uint32_t)(p.half_dn ? p.half_dn : p.bn)};
-  return encode_map(m, base, 4, dims, str, box, f32 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : map_dtype(dt),
+  return encode_map(m, base, 4, dims, str, box, f32 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : tma_dtype(dt),
                     CU_TENSOR_MAP_SWIZZLE_32B);
 }
 
@@ -550,8 +464,6 @@ int32_t launch_tc(int32_t dt, const CUtensorMap& ma, const CUtensorMap& mw, cons
 
 }  // namespace
 
-extern "C" int32_t fyc_tcgen05_available(void) { return get_encode_fn() != nullptr ? 1 : 0; }
-
 // Is this GEMM eligible for the tensor-core path?
 bool fyc_gemm_tc_eligible(const fyc_gemm_args* g) {
   if (!fyc_is_16bit(g->dtype)) return false;
@@ -573,7 +485,7 @@ bool fyc_gemm_tc_eligible(const fyc_gemm_args* g) {
   if ((g->epilogue & FYC_EPI_BIAS) && ((uintptr_t)g->bias & 15)) return false;
   if ((g->epilogue & FYC_EPI_ROWBIAS) && ((uintptr_t)g->rowbias & 15)) return false;
   (void)n_out;
-  return get_encode_fn() != nullptr;
+  return tma_available();
 }
 
 int32_t fyc_gemm_tc(const fyc_gemm_args* g, cudaStream_t st) {
@@ -590,14 +502,14 @@ int32_t fyc_gemm_tc(const fyc_gemm_args* g, cudaStream_t st) {
       uint64_t dims[4] = {(uint64_t)Ka, (uint64_t)g->M, 1, 1};
       uint64_t str[3] = {(uint64_t)g->lda * 2, (uint64_t)g->lda * 2 * (uint64_t)g->M, (uint64_t)g->lda * 2 * (uint64_t)g->M};
       uint32_t box[4] = {BK, BM, 1, 1};
-      int32_t rc = encode_map(&ma, A, 4, dims, str, box, map_dtype(g->dtype));
+      int32_t rc = encode_map(&ma, A, 4, dims, str, box, tma_dtype(g->dtype));
       if (rc) return rc;
     }
     if (g->A2) {
       uint64_t dims[4] = {(uint64_t)(g->K - g->K1), (uint64_t)g->M, 1, 1};
       uint64_t str[3] = {(uint64_t)g->lda2 * 2, (uint64_t)g->lda2 * 2 * (uint64_t)g->M, (uint64_t)g->lda2 * 2 * (uint64_t)g->M};
       uint32_t box[4] = {BK, BM, 1, 1};
-      int32_t rc = encode_map(&ma2, g->A2, 4, dims, str, box, map_dtype(g->dtype));
+      int32_t rc = encode_map(&ma2, g->A2, 4, dims, str, box, tma_dtype(g->dtype));
       if (rc) return rc;
     }
     TcParams p{};
@@ -613,7 +525,7 @@ int32_t fyc_gemm_tc(const fyc_gemm_args* g, cudaStream_t st) {
       uint64_t dims[3] = {(uint64_t)g->K, 1, (uint64_t)g->N};
       uint64_t str[2] = {(uint64_t)g->ldw * 2, (uint64_t)g->ldw * 2};
       uint32_t box[3] = {BK, 1, (uint32_t)p.BN};
-      int32_t rc = encode_map(&mw, W, 3, dims, str, box, map_dtype(g->dtype));
+      int32_t rc = encode_map(&mw, W, 3, dims, str, box, tma_dtype(g->dtype));
       if (rc) return rc;
     }
     FYC_CHECK(g->M < (1ll << 31), "gemm(tensor cores): M too large");
@@ -658,7 +570,7 @@ bool fyc_conv3x3_tc_eligible(const fyc_conv3x3_args* c) {
   if (c->epilogue & FYC_EPI_GEGLU) return false;
   int bw, bh, bn;
   if (!pick_patch(c->NB, c->H / c->stride, c->W / c->stride, &bw, &bh, &bn)) return false;
-  return get_encode_fn() != nullptr;
+  return tma_available();
 }
 
 // x for stride 2 must already be the parity-plane split (see fyc_space_to_planes); H, W are the ORIGINAL dims.
@@ -696,14 +608,14 @@ int32_t fyc_conv3x3_tc(const fyc_conv3x3_args* c, const void* x_planes, cudaStre
     uint64_t dims[4] = {(uint64_t)c->Cin, (uint64_t)Wo, (uint64_t)Ho, imgs};
     uint64_t str[3] = {(uint64_t)c->Cin * 2, (uint64_t)c->Cin * 2 * Wo, (uint64_t)c->Cin * 2 * Wo * Ho};
     uint32_t box[4] = {BK, (uint32_t)p.bw, (uint32_t)p.bh, (uint32_t)p.bn};
-    int32_t rc = encode_map(&ma, xa, 4, dims, str, box, map_dtype(c->dtype));
+    int32_t rc = encode_map(&ma, xa, 4, dims, str, box, tma_dtype(c->dtype));
     if (rc) return rc;
   }
   {
     uint64_t dims[3] = {(uint64_t)c->Cin, 9, (uint64_t)c->Cout};
     uint64_t str[2] = {(uint64_t)c->Cin * 2, (uint64_t)c->Cin * 2 * 9};
     uint32_t box[3] = {BK, 1, (uint32_t)p.BN};
-    int32_t rc = encode_map(&mw, c->w, 3, dims, str, box, map_dtype(c->dtype));
+    int32_t rc = encode_map(&mw, c->w, 3, dims, str, box, tma_dtype(c->dtype));
     if (rc) return rc;
   }
   p.bias = c->bias; p.rowbias = c->rowbias;
@@ -734,7 +646,7 @@ bool fyc_conv3x3_up2_tc_eligible(const fyc_conv3x3_args* c) {
   if (c->epilogue & ~FYC_EPI_BIAS) return false;          // the upsamplers carry a bias only (resnet.py:168, diffusers resnet.py:139)
   int bw, bh, bn;
   if (!pick_patch(c->NB, c->H, c->W, &bw, &bh, &bn)) return false;
-  return get_encode_fn() != nullptr;
+  return tma_available();
 }
 
 int32_t fyc_conv3x3_up2_tc(const fyc_conv3x3_args* c, cudaStream_t st) {
@@ -756,7 +668,7 @@ int32_t fyc_conv3x3_up2_tc(const fyc_conv3x3_args* c, cudaStream_t st) {
     uint64_t dims[4] = {(uint64_t)c->Cin, (uint64_t)W, (uint64_t)H, (uint64_t)c->NB};
     uint64_t str[3] = {(uint64_t)c->Cin * 2, (uint64_t)c->Cin * 2 * W, (uint64_t)c->Cin * 2 * W * H};
     uint32_t box[4] = {BK, (uint32_t)p.bw, (uint32_t)p.bh, (uint32_t)p.bn};
-    int32_t rc = encode_map(&ma, c->x, 4, dims, str, box, map_dtype(c->dtype));
+    int32_t rc = encode_map(&ma, c->x, 4, dims, str, box, tma_dtype(c->dtype));
     if (rc) return rc;
   }
   for (int ph = 0; ph < 4; ++ph) {
@@ -769,7 +681,7 @@ int32_t fyc_conv3x3_up2_tc(const fyc_conv3x3_args* c, cudaStream_t st) {
     uint64_t dims[3] = {(uint64_t)c->Cin, 4, (uint64_t)c->Cout};
     uint64_t str[2] = {(uint64_t)c->Cin * 2, (uint64_t)c->Cin * 2 * 4};
     uint32_t box[3] = {BK, 1, (uint32_t)p.BN};
-    int32_t rc = encode_map(&mw, wp, 3, dims, str, box, map_dtype(c->dtype));
+    int32_t rc = encode_map(&mw, wp, 3, dims, str, box, tma_dtype(c->dtype));
     if (rc) return rc;
     const uint64_t C = (uint64_t)c->Cout;
     CUtensorMap mo;

@@ -7,24 +7,6 @@
 
 namespace {
 
-__device__ __forceinline__ void cp_async16(void* dst, const void* src) {
-  unsigned d = (unsigned)__cvta_generic_to_shared(dst);
-  asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(d), "l"(src) : "memory");
-}
-__device__ __forceinline__ void ldsm4(uint32_t* r, const void* p) {
-  unsigned a = (unsigned)__cvta_generic_to_shared(p);
-  asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0, %1, %2, %3}, [%4];" : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]) : "r"(a));
-}
-__device__ __forceinline__ void ldsm4t(uint32_t* r, const void* p) {
-  unsigned a = (unsigned)__cvta_generic_to_shared(p);
-  asm volatile("ldmatrix.sync.aligned.m8n8.x4.trans.shared.b16 {%0, %1, %2, %3}, [%4];" : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]) : "r"(a));
-}
-__device__ __forceinline__ float ex2_approx(float x) {
-  float y;
-  asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
-  return y;
-}
-
 // FP = frames padded to 16 or 32; DP = head dim padded to a multiple of 16; T = the 16-bit storage type (bf16 | f16)
 template <int FP, int DP, typename T>
 __global__ void __launch_bounds__(256) temporal_attention_mma_kernel(const T* __restrict__ qkv, T* __restrict__ out, int64_t B,
@@ -54,7 +36,8 @@ __global__ void __launch_bounds__(256) temporal_attention_mma_kernel(const T* __
     if (r < F && (i % ch) < chv) cp_async16(dst, src + (int64_t)r * row_stride + seg * C + c);
     else *reinterpret_cast<uint4*>(dst) = make_uint4(0, 0, 0, 0);
   }
-  asm volatile("cp.async.commit_group;\ncp.async.wait_group 0;" ::: "memory");
+  cp_async_commit();
+  cp_async_wait<0>();
   __syncwarp();
   const int g = lane >> 2, t = lane & 3, mi = lane >> 3;
 #pragma unroll
@@ -65,11 +48,11 @@ __global__ void __launch_bounds__(256) temporal_attention_mma_kernel(const T* __
 #pragma unroll
     for (int ks = 0; ks < KS; ++ks) {
       uint32_t a[4];
-      ldsm4(a, sq + (mt * 16 + (lane & 15)) * LDS + ks * 16 + (lane >> 4) * 8);
+      ldmatrix_x4(a, sq + (mt * 16 + (lane & 15)) * LDS + ks * 16 + (lane >> 4) * 8);
 #pragma unroll
       for (int jp = 0; jp < NT / 2; ++jp) {
         uint32_t bb[4];
-        ldsm4(bb, sk + (jp * 16 + (lane & 7) + (mi >> 1) * 8) * LDS + ks * 16 + (mi & 1) * 8);
+        ldmatrix_x4(bb, sk + (jp * 16 + (lane & 7) + (mi >> 1) * 8) * LDS + ks * 16 + (mi & 1) * 8);
         mma16816<T>(s[2 * jp], a, bb[0], bb[1]);
         mma16816<T>(s[2 * jp + 1], a, bb[2], bb[3]);
       }
@@ -107,7 +90,7 @@ __global__ void __launch_bounds__(256) temporal_attention_mma_kernel(const T* __
 #pragma unroll
       for (int kk = 0; kk < KK; ++kk) {
         uint32_t bb[4];
-        ldsm4t(bb, sv + (kk * 16 + (lane & 7) + (mi & 1) * 8) * LDS + np * 16 + (mi >> 1) * 8);
+        ldmatrix_x4_trans(bb, sv + (kk * 16 + (lane & 7) + (mi & 1) * 8) * LDS + np * 16 + (mi >> 1) * 8);
         mma16816<T>(o[0], pf[kk], bb[0], bb[1]);
         mma16816<T>(o[1], pf[kk], bb[2], bb[3]);
       }
