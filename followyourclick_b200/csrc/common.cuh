@@ -192,6 +192,8 @@ __device__ __forceinline__ float ex2_approx(float x) {
 // |gelu error| <= 1.3e-6 over all x; fit script in DESIGN.md): ONE MUFU.EX2 + 7 FMAs instead of erff()'s ~30 instructions.
 // (A first version with Abramowitz-Stegun 7.1.26 needed rcp + ex2 = two MUFU ops per element and made the GEGLU epilogue
 // MUFU-bound: 431 vs 636 TFLOP/s on the level-0 FF1 GEMM.)
+// |gelu_erf_fast(x) - gelu(x)| <= 1.3e-6 + 2^-23 |x| (polynomial and ex2.approx measured on a dense grid over [-12, 12], plus fp32
+// rounding); fminf drops a NaN x, the final multiply by x still returns NaN.
 __device__ __forceinline__ float gelu_erf_fast(float x) {
   const float z = fminf(fabsf(x) * 0.70710678118654752440f, 4.0f);
   float q = fmaf(-0.002980560529977083f, z, 0.02972414717078209f);

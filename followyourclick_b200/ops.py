@@ -211,6 +211,10 @@ def gemm(A, W, bias=None, residual=None, rowbias=None, rows_per_group=0, alpha=1
     assert W.shape[-1] == K and W.dtype == A.dtype
     fused_geglu = geglu and impl != L.IMPL_SIMT and tc_ok(A.dtype, M)
     n_out = N // 2 if fused_geglu else N
+    if geglu and not fused_geglu and out is not None and not out.is_contiguous():
+        # fyc_geglu writes packed [M, N / 2] rows: a wider row stride would put rows in the wrong place and write outside the view
+        raise L.FycError("gemm: the unfused GEGLU epilogue (CUDA-core path) writes a contiguous output; got row stride "
+                         f"{out.stride(-2)} for {N // 2} columns")
     odt = torch.float32 if out_f32 else A.dtype
     if out is None or (geglu and not fused_geglu):
         o = torch.empty((Bn, M, n_out) if batched else (M, n_out), dtype=odt, device=A.device)

@@ -203,7 +203,9 @@ int32_t fyc_self_attention_tc_d80_f16(const void* qkv, int64_t ldqkv, int64_t q_
  * One CTA per (image, head) keeps K, V^T (and K2, V2^T) in shared memory and ping-pongs two softmax warpgroups over its query tiles; S and
  * O live in registers, the probabilities are normalised in registers (one key tile: no online rescaling) and both contexts accumulate into ONE
  * O accumulator, written once.  Operands, packed once per clip by the caller:
- *   q   [NB, Lq, ldq], head h at columns [q_col0 + D h, +D), unpadded;
+ *   q   [NB, Lq, ldq], head h at columns [q_col0 + D h, +D), unpadded (for D = 40 the 64-column q box of head h also holds the first 24
+ *       columns of head h + 1, which meet the zero key columns 40..63: a NaN in those columns of head h + 1 makes head h's row NaN too;
+ *       the box of the last head ends at column heads D, past which nothing is read);
  *   k   [NBc, 80, ldk], head h at columns [DKP h, +D) with DKP = 64 for D = 40 (columns D..63 of every head ZERO) | 64 for D = 64 | 80 for
  *       D = 80, rows Lk..79 zero;
  *   vt  [NBc, heads D, 80] (V transposed: keys contiguous), columns Lk..79 zero;
