@@ -55,6 +55,7 @@ SIGNATURES = {
     "fyc_conv3x3_workspace_bytes": (_sz, [C.POINTER(ConvArgs)]),
     "fyc_conv3x3": (_i32, [C.POINTER(ConvArgs), _vp]),
     "fyc_conv3x3_up2_eligible": (_i32, [C.POINTER(ConvArgs)]),
+    "fyc_conv3x3_tc_route": (_i32, [C.POINTER(ConvArgs)]),
     "fyc_groupnorm_workspace_bytes": (_sz, [_i64, _i64, _i64]),
     "fyc_groupnorm": (_i32, [_vp, _vp, _vp, _vp, _i64, _i64, _i64, _i64, _f32, _i32, _i32, _vp, _sz, _vp]),
     "fyc_groupnorm_concat": (_i32, [_vp, _i64, _vp, _i64, _vp, _vp, _vp, _i64, _i64, _i64, _f32, _i32, _i32, _vp, _sz, _vp]),

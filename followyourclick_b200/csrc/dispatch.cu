@@ -49,6 +49,20 @@ extern "C" int32_t fyc_conv3x3_up2_eligible(const fyc_conv3x3_args* c) {
   return (c && c->impl != FYC_IMPL_SIMT && fyc_tcgen05_available() == 1 && fyc_conv3x3_up2_tc_eligible(c)) ? 1 : 0;
 }
 
+// The route of a fyc_conv3x3 call (workspace as given): the one rule for both the launch below and fyc_conv3x3_tc_route.
+enum ConvRoute { CONV_SIMT, CONV_TC, CONV_TC_UP2 };
+static ConvRoute conv3x3_route(const fyc_conv3x3_args* c) {
+  if (c->impl == FYC_IMPL_SIMT) return CONV_SIMT;
+  if (c->upsample == 2 && c->w_phases && fyc_conv3x3_up2_tc_eligible(c)) return CONV_TC_UP2;
+  if (!fyc_conv3x3_tc_eligible(c)) return CONV_SIMT;
+  if (c->stride == 2 && (!c->workspace || c->workspace_bytes < fyc_conv3x3_workspace_bytes(c))) return CONV_SIMT;
+  return CONV_TC;
+}
+
+extern "C" int32_t fyc_conv3x3_tc_route(const fyc_conv3x3_args* c) {
+  return (c && conv3x3_route(c) != CONV_SIMT) ? 1 : 0;
+}
+
 extern "C" int32_t fyc_conv3x3(const fyc_conv3x3_args* c, void* stream) {
   cudaStream_t st = (cudaStream_t)stream;
   FYC_CHECK(c && c->x && c->w && c->out, "conv3x3: null pointer");
@@ -59,15 +73,15 @@ extern "C" int32_t fyc_conv3x3(const fyc_conv3x3_args* c, void* stream) {
   FYC_CHECK(!(c->epilogue & FYC_EPI_BIAS) || c->bias, "conv3x3: FYC_EPI_BIAS without bias");
   FYC_CHECK(!(c->epilogue & FYC_EPI_RESIDUAL) || c->residual, "conv3x3: FYC_EPI_RESIDUAL without residual");
   FYC_CHECK(!(c->epilogue & FYC_EPI_ROWBIAS) || (c->rowbias && c->images_per_group > 0), "conv3x3: FYC_EPI_ROWBIAS without rowbias");
-  if (c->impl != FYC_IMPL_SIMT && c->upsample == 2 && c->w_phases && fyc_conv3x3_up2_tc_eligible(c)) return fyc_conv3x3_up2_tc(c, st);
-  bool tc = (c->impl != FYC_IMPL_SIMT) && fyc_conv3x3_tc_eligible(c);
-  if (tc && c->stride == 2 && (!c->workspace || c->workspace_bytes < fyc_conv3x3_workspace_bytes(c))) {
-    FYC_CHECK(c->impl != FYC_IMPL_TCGEN05, "conv3x3(tensor cores): stride-2 needs %zu workspace bytes", fyc_conv3x3_workspace_bytes(c));
-    tc = false;
+  const ConvRoute route = conv3x3_route(c);
+  if (route == CONV_TC_UP2) return fyc_conv3x3_up2_tc(c, st);
+  if (route == CONV_SIMT) {
+    FYC_CHECK(c->impl != FYC_IMPL_TCGEN05 || c->stride != 2 || !fyc_conv3x3_tc_eligible(c),
+              "conv3x3(tensor cores): stride-2 needs %zu workspace bytes", fyc_conv3x3_workspace_bytes(c));
+    FYC_CHECK(c->impl != FYC_IMPL_TCGEN05, "conv3x3: tensor-core path requested but shape not eligible");
+    if (c->impl == FYC_IMPL_AUTO && fyc_conv_small_n_eligible(c)) return fyc_conv_small_n(c, st);
+    return fyc_conv3x3_simt(c, st);
   }
-  FYC_CHECK(tc || c->impl != FYC_IMPL_TCGEN05, "conv3x3: tensor-core path requested but shape not eligible");
-  if (!tc && c->impl == FYC_IMPL_AUTO && fyc_conv_small_n_eligible(c)) return fyc_conv_small_n(c, st);
-  if (!tc) return fyc_conv3x3_simt(c, st);
   if (c->stride == 2) {
     int32_t rc = fyc_space_to_planes(c->x, c->workspace, c->NB, c->H, c->W, c->Cin, st);
     if (rc) return rc;

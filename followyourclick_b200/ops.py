@@ -291,7 +291,8 @@ def conv3x3(x, w, bias=None, residual=None, rowbias=None, images_per_group=0, st
     if nbytes:
         ws = torch.empty(nbytes, dtype=torch.uint8, device=x.device)
         a.workspace, a.workspace_bytes = ptr(ws), nbytes
-    fam = "conv_tc" if (impl != L.IMPL_SIMT and tc_ok(x.dtype, NB * Ho * Wo) and Cin % 8 == 0 and Cout % 16 == 0) else "conv_simt"
+    # the label names the kernel fyc_conv3x3 runs: channel counts alone do not decide it (a 5 x 9 grid has no 128-pixel patch)
+    fam = "conv_tc" if lib().fyc_conv3x3_tc_route(C.byref(a)) == 1 else "conv_simt"
     if _prof_shapes:
         fam += f"[{NB}x{Ho}x{Wo} {Cin}->{Cout} s{stride}]"
     with _rec(fam, 2.0 * NB * Ho * Wo * Cout * 9 * Cin, x.element_size() * (x.numel() + w.numel() + out.numel())):

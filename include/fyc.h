@@ -119,6 +119,10 @@ int32_t fyc_conv3x3(const fyc_conv3x3_args* a, void* stream);
 /* 1 when a (upsample == 2, w_phases != NULL) call will take the four-phase tensor-core path, else 0 (the caller then either
  * materialises the upsample and runs the plain 3x3 path, or lets fyc_conv3x3 fold it into the CUDA-core kernel's index). */
 int32_t fyc_conv3x3_up2_eligible(const fyc_conv3x3_args* a);
+/* 1 when fyc_conv3x3 will run this call (workspace as given) on the tensor-core kernel, else 0 (the CUDA-core kernels).  A shape whose
+ * output grid has no 128-pixel patch bw x bh x bn of powers of two dividing Wo, Ho and NB (e.g. 5 x 9 pixels over 32 images) is not
+ * tensor-core eligible even when its channel counts are. */
+int32_t fyc_conv3x3_tc_route(const fyc_conv3x3_args* a);
 
 /* ---- normalisation ------------------------------------------------------------------------------------
  * GroupNorm (+ optional SiLU) over x viewed as [NB, R, C]: statistics per (nb, group) over R rows x C/G

@@ -143,12 +143,12 @@ def _f64(ops_in):
     return {n: t.double() for n, t in ops_in.items()}
 
 
-def ref64(case, operands=None):
-    return REF[case.op](_f64(case.operands if operands is None else operands), **case.params)
+def ref64(case, operands=None, elems=None):
+    return _blocked(REF[case.op], case, case.operands if operands is None else operands, elems)
 
 
-def mag64(case):
-    return MAG[case.op](_f64(case.operands), **case.params)
+def mag64(case, elems=None):
+    return _blocked(MAG[case.op], case, case.operands, elems)
 
 
 def check_surround(out_nan, out_zero, frames_nan, frames_zero):
@@ -451,9 +451,11 @@ def cross_tc_mag(o, **p):
     return _cross_tc(o, absterm=True, **p)[1]
 
 
-def _self_tc(o, heads, D, scale, q_col0, k_col0, hstride, u_s=0.0, absterm=False, **_):
+def _self_tc(o, heads, D, scale, q_col0, k_col0, hstride, u_s=0.0, absterm=False, q_rows=None, **_):
+    """``q_rows`` (lo, hi): only the outputs of query rows lo..hi - 1 (every key still attends)"""
     qk = o["qk"]
-    q, k = _heads(qk[:, :, q_col0:], heads, D, hstride), _heads(qk[:, :, k_col0:], heads, D, hstride)
+    qr = qk if q_rows is None else qk[:, q_rows[0]:q_rows[1]]
+    q, k = _heads(qr[:, :, q_col0:], heads, D, hstride), _heads(qk[:, :, k_col0:], heads, D, hstride)
     vt = o["vt"]
     v = vt.reshape(vt.shape[0], heads, D, -1).transpose(-1, -2)
     y, m = _softmax_pv(q, k, v, scale, u_s, absterm)
@@ -508,6 +510,92 @@ REF = dict(gemm=gemm_ref, conv=conv_ref, groupnorm=groupnorm_ref, layernorm=laye
            cross_tc=cross_tc_ref, self_tc=self_tc_ref, temporal=temporal_ref, transpose=transpose_ref, softmax=softmax_ref)
 MAG = dict(gemm=gemm_mag, conv=conv_mag, groupnorm=groupnorm_mag, layernorm=layernorm_mag, lnstats=lnstats_mag, attention=attention_mag,
            cross_tc=cross_tc_mag, self_tc=self_tc_mag, temporal=temporal_mag, transpose=transpose_mag, softmax=softmax_mag)
+
+
+# ---- the references in blocks of output rows ----------------------------------------------------------------------------------
+# A block's largest fp64 intermediate (attention scores, a conv's im2col matrix, a GEMM's pre-activation) holds about CHUNK_ELEMS
+# elements (256 MB); the few such tensors alive at once keep a case within ~4 GB of device memory at any shape.  Output rows are
+# independent in every chunked operation, so the blocks concatenate to the unchunked result.
+
+CHUNK_ELEMS = 1 << 25
+
+
+def _blocks(n, per_row, align, elems):
+    step = max(align, (elems // max(per_row, 1)) // align * align)
+    return [(lo, min(lo + step, n)) for lo in range(0, n, step)]
+
+
+def _rows(t, axis, lo, hi):
+    return t.narrow(axis % t.dim(), lo, hi - lo)
+
+
+def _group_rows(t, lo, hi, per):
+    """rows of a per-group table (row bias) that serve items lo..hi - 1, ``per`` items a group, lo a multiple of ``per``"""
+    return t[lo // per:-(-hi // per)]
+
+
+def _split_gemm(o, p, elems):
+    A = o["A"]
+    M = A.shape[-2]
+    rpg = p.get("rows_per_group", 0) if "rowbias" in o else 0
+    per_row = (o["W"].shape[-2] + A.shape[-1]) * (A.shape[0] if A.dim() == 3 else 1)
+    out = []
+    for lo, hi in _blocks(M, per_row, max(rpg, 1), elems):
+        b = {n: (_rows(t, -2, lo, hi) if n in ("A", "A2", "residual") else t) for n, t in o.items()}
+        if "ln" in o:
+            b["ln"] = o["ln"][lo:hi]
+        if rpg:
+            b["rowbias"] = _group_rows(o["rowbias"], lo, hi, rpg)
+        out.append((b, p))
+    return -2, out
+
+
+def _split_conv(o, p, elems):
+    NB, H, W, Cin = o["x"].shape
+    ipg = p.get("images_per_group", 1)
+    up = p.get("upsample", 1)
+    Cout = o["w_phases"].shape[1] if "w_phases" in o else o["w"].shape[0]
+    per_img = H * W * up * up * (9 * Cin + Cout)
+    out = []
+    for lo, hi in _blocks(NB, per_img, ipg if "rowbias" in o else 1, elems):
+        b = {n: (t[lo:hi] if n in ("x", "residual") else t) for n, t in o.items()}
+        if "rowbias" in o:
+            b["rowbias"] = _group_rows(o["rowbias"], lo, hi, ipg)
+        out.append((b, p))
+    return 0, out
+
+
+def _split_query(key_rows):
+    """attention over query rows (operand "q", axis 1) against every key: the block holds rows x (batch heads keys) scores"""
+    def split(o, p, elems):
+        q = o["q"]
+        per_row = q.shape[0] * p["heads"] * key_rows(o, p)
+        out = []
+        for lo, hi in _blocks(q.shape[1], per_row, 1, elems):
+            out.append(({n: (t[:, lo:hi] if n in ("q", "out0") else t) for n, t in o.items()}, p))
+        return 1, out
+    return split
+
+
+def _split_self_tc(o, p, elems):
+    NB, L = o["qk"].shape[:2]
+    return 1, [(o, dict(p, q_rows=(lo, hi))) for lo, hi in _blocks(L, NB * p["heads"] * L, 1, elems)]
+
+
+SPLIT = dict(gemm=_split_gemm, conv=_split_conv, self_tc=_split_self_tc,
+             attention=_split_query(lambda o, p: o["k"].shape[1] + (o["k2"].shape[1] if "k2" in o else 0)),
+             cross_tc=_split_query(lambda o, p: p["Lk"] + p.get("Lk2", 0)))
+
+
+def _blocked(fn, case, operands, elems=None):
+    """fn (a REF or MAG entry) on the fp64 operands, one block of output rows at a time"""
+    split = SPLIT.get(case.op)
+    if split is None:
+        return fn(_f64(operands), **case.params)
+    axis, blocks = split(operands, case.params, CHUNK_ELEMS if elems is None else elems)
+    if len(blocks) == 1:
+        return fn(_f64(operands), **case.params)
+    return torch.cat([fn(_f64(b), **p) for b, p in blocks], dim=axis)
 
 
 # ---- case builders (shared by the GPU test and its CPU self-test) -----------------------------------------------------------------
@@ -659,12 +747,43 @@ def layernorm_case(dtype, M, C, device, pe=False, stats_only=False, name=None):
                 out_dtype=torch.float32 if stats_only else dtype, device=device)
 
 
-def attention_case(dtype, heads, D, B, Lq, Lk, div, device, T=0, accumulate=False, impl=None, name=None):
+LAYOUTS = ("gaussian", "ascending", "late_peak", "flat")
+SPAN = 30.0                   # logit range of the ascending and late-peak layouts
+
+
+def layout_qk(layout, N, L, heads, D, scale):
+    """self-attention q, k [N, L, heads, D] fp32 (cpu) whose scores have a given structure:
+    gaussian  - independent N(0, 1) entries;
+    ascending - every row's score rises with the key index (0 .. ~SPAN): each key tile raises the running max of the online softmax;
+    late_peak - key L - 2, in the last key tile, exceeds every other score of every row by ~SPAN;
+    flat      - every key row is the same: a row's scores are all equal, the normaliser sums over every tile."""
+    q, k = rnd((N, L, heads, D), 1, torch.float32, "cpu"), rnd((N, L, heads, D), 2, torch.float32, "cpu")
+    if layout == "ascending":
+        # q0 in [3, 4) per row and head, q1.. zero: s = scale q0 k0, k0 a ramp that reaches SPAN at q0 = 4
+        q = torch.cat([3 + rnd((N, L, heads, 1), 3, torch.float32, "cpu").abs().clamp(max=0.99), torch.zeros(N, L, heads, D - 1)], dim=-1)
+        k[..., 0] = torch.linspace(0, SPAN / (4 * scale), L)[None, :, None]
+    elif layout == "late_peak":
+        q, k = 0.5 * q, 0.5 * k
+        q[..., 0], k[..., 0] = 4.0, 0.0
+        k[:, L - 2, :, 0] = SPAN / (4 * scale)
+    elif layout == "flat":
+        k = k[:, :1].expand(N, L, heads, D).contiguous()
+    else:
+        assert layout == "gaussian", layout
+    return q, k
+
+
+def attention_case(dtype, heads, D, B, Lq, Lk, div, device, T=0, accumulate=False, impl=None, layout="gaussian", name=None):
     """ops.attention on strided q / k / v views (rows wider than the heads), context n / div, optional fused second context of T keys,
-    or the accumulate form (out = out0 + out_alpha softmax(..) v, out0 a finite prefill)"""
+    or the accumulate form (out = out0 + out_alpha softmax(..) v, out0 a finite prefill); ``layout``: a score structure of layout_qk
+    (self-attention shapes: Lq = Lk, div = 1)"""
     from followyourclick_b200 import _lib
     C, Bc = heads * D, B // div
     o = dict(q=rnd((B, Lq, C), 1, dtype, device), k=rnd((Bc, Lk, C), 2, dtype, device), v=rnd((Bc, Lk, C), 3, dtype, device))
+    if layout != "gaussian":
+        assert Lq == Lk and div == 1
+        q, k = layout_qk(layout, B, Lq, heads, D, D ** -0.5)
+        o["q"], o["k"] = q.reshape(B, Lq, C).to(dtype).to(device), k.reshape(B, Lk, C).to(dtype).to(device)
     if T:
         o["k2"], o["v2"] = rnd((Bc, T, C), 4, dtype, device), rnd((Bc, T, C), 5, dtype, device)
     if accumulate:
@@ -719,14 +838,18 @@ def cross_tc_case(dtype, heads, D, NB, Lq, Lk, T, div, device, name=None):
                 out_dtype=dtype, device=device)
 
 
-def self_tc_case(dtype, D, NB, L, heads, device, wide_out=True, name=None):
+def self_tc_case(dtype, D, NB, L, heads, device, wide_out=True, layout="gaussian", name=None):
     """fyc_self_attention_tc (D 40 / 64: 64-wide q / k heads, D = 40 columns 40..63 zero) or fyc_self_attention_tc_d80 (unpadded heads of
     the fused projection: the operand is the [q | k] part, the v block of the row is poison the kernel must not read).  ``wide_out``:
-    output rows wider than the heads - a row stride ops does not expose, so the entry point is called directly."""
+    output rows wider than the heads - a row stride ops does not expose, so the entry point is called directly.  ``layout``: the score
+    structure of layout_qk."""
     from followyourclick_b200 import _lib
     C = heads * D
     hs = 80 if D == 80 else 64
-    q, k = rnd((NB, L, heads, D), 1, dtype, "cpu"), rnd((NB, L, heads, D), 2, dtype, "cpu")
+    if layout == "gaussian":
+        q, k = rnd((NB, L, heads, D), 1, dtype, "cpu"), rnd((NB, L, heads, D), 2, dtype, "cpu")
+    else:
+        q, k = (t.to(dtype) for t in layout_qk(layout, NB, L, heads, D, D ** -0.5))
     qk = torch.zeros((NB, L, 2, heads, hs), dtype=dtype)
     qk[:, :, 0, :, :D], qk[:, :, 1, :, :D] = q, k
     o = dict(qk=qk.reshape(NB, L, 2 * heads * hs).to(device), vt=rnd((NB, C, L), 3, dtype, device))
