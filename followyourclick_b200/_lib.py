@@ -82,6 +82,8 @@ SIGNATURES = {
     "fyc_ncfhw_to_nfhwc": (_i32, [_vp, _vp, _i64, _i64, _i64, _i64, _f32, _i32, _vp]),
     "fyc_nfhwc_to_ncfhw": (_i32, [_vp, _vp, _i64, _i64, _i64, _i64, _i64, _i32, _vp]),
     "fyc_build_unet_input": (_i32, [_vp, _vp, _vp, _vp, _i64, _i64, _i64, _i32, _i32, _i32, _vp]),
+    "fyc_build_unet_input_first": (_i32, [_vp, _vp, _vp, _i64, _i64, _i64, _i32, _i32, _i32, _i32, _vp]),
+    "fyc_first_frame_temb_rows": (_i32, [_vp, _vp, _i64, _i64, _i64, _vp]),
     "fyc_cfg_ddim_step": (_i32, [_vp, _vp, _vp, _vp, _i64, C.POINTER(DdimCoefs), _vp]),
     "fyc_cfg_video_ddim_step": (_i32, [_vp, _vp, _f32, _vp, _vp, _vp, _i64, C.POINTER(DdimCoefs), _vp]),
     "fyc_frames_finalize": (_i32, [_vp, _vp, _i64, _i64, _i64, _i64, _i32, _vp]),

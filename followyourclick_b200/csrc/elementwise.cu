@@ -208,6 +208,60 @@ extern "C" int32_t fyc_build_unet_input(const float* latents, const float* mask,
   return FYC_OK;
 }
 
+// The first-frame-conditioned models' step prologue (fyc.h fyc_build_unet_input_first).  One thread per pixel (clip, frame, position):
+// under FYC_FIRST_FRAME the frame-0 threads overwrite their own four latents with the first-image latents before reading them, so no
+// thread reads what another one writes.
+template <typename T>
+__global__ void build_unet_input_first_kernel(float* __restrict__ lat, const float* __restrict__ first, T* __restrict__ out, int64_t b,
+                                              int64_t F, int64_t HW, int dup, int mode, int c_pad) {
+  const int Cin = (mode & FYC_FIRST_CONCAT) ? 8 : 4;
+  int64_t total = b * F * HW;
+  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
+    int64_t p = i % HW; int64_t r = i / HW;
+    int64_t f = r % F; int64_t bi = r / F;
+    float v[8];
+#pragma unroll
+    for (int c = 0; c < 4; ++c) {
+      float* src = lat + ((bi * 4 + c) * F + f) * HW + p;
+      if ((mode & FYC_FIRST_FRAME) && f == 0) *src = first[(bi * 4 + c) * HW + p];
+      v[c] = *src;
+      v[4 + c] = first[(bi * 4 + c) * HW + p];
+    }
+    for (int d = 0; d < dup; ++d) {
+      T* o = out + (((d * b + bi) * F + f) * HW + p) * c_pad;
+      for (int c = 0; c < Cin; ++c) o[c] = from_f<T>(v[c]);
+      for (int c = Cin; c < c_pad; ++c) o[c] = from_f<T>(0.f);
+    }
+  }
+}
+extern "C" int32_t fyc_build_unet_input_first(float* latents, const float* first, void* out, int64_t b, int64_t F, int64_t HW, int32_t dup,
+                                              int32_t mode, int32_t c_pad, int32_t dtype, void* stream) {
+  FYC_CHECK(latents && first && out && b > 0 && F > 0 && HW > 0, "build_unet_input_first: bad arguments");
+  FYC_CHECK(dup == 1 || dup == 2, "build_unet_input_first: dup must be 1 or 2");
+  FYC_CHECK(mode >= 1 && mode <= (FYC_FIRST_CONCAT | FYC_FIRST_FRAME), "build_unet_input_first: unknown mode %d", mode);
+  FYC_CHECK(c_pad >= ((mode & FYC_FIRST_CONCAT) ? 8 : 4) && c_pad <= 64, "build_unet_input_first: c_pad=%d", c_pad);
+  FYC_DISPATCH(dtype, build_unet_input_first_kernel<T><<<grid_for(b * F * HW, 256), 256, 0, (cudaStream_t)stream>>>(latents, first, (T*)out, b, F, HW, dup, mode, c_pad));
+  FYC_LAUNCH_CHECK();
+  return FYC_OK;
+}
+
+// Per-image time-embedding rows of the first-frame condition (resnet.py:304-313): frame 0 of every clip reads row B (the t = 0 row the
+// UNet appends, unet.py:523-524), frame f > 0 of clip b reads row b.
+__global__ void first_frame_temb_rows_kernel(const float* __restrict__ temb, float* __restrict__ out, int64_t B, int64_t F, int64_t N) {
+  const int64_t total = B * F * N;
+  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
+    const int64_t n = i % N, img = i / N;
+    const int64_t f = img % F, bi = img / F;
+    out[i] = temb[(f == 0 ? B : bi) * N + n];
+  }
+}
+extern "C" int32_t fyc_first_frame_temb_rows(const float* temb, float* out, int64_t B, int64_t F, int64_t N, void* stream) {
+  FYC_CHECK(temb && out && B > 0 && F > 0 && N > 0, "first_frame_temb_rows: bad arguments");
+  first_frame_temb_rows_kernel<<<grid_for(B * F * N, 256), 256, 0, (cudaStream_t)stream>>>(temb, out, B, F, N);
+  FYC_LAUNCH_CHECK();
+  return FYC_OK;
+}
+
 // ---------------------------------------------------------------------------------------------------------
 // CFG combine + DDIM step.  Operation order and roundings follow the reference line by line so that the fp32
 // result is bit-identical to PyTorch eager (each torch op rounds once; no FMA contraction):

@@ -560,6 +560,36 @@ def build_unet_input(latents, mask, first, dup, dtype, c_pad=None, out=None):
     return out
 
 
+FIRST_CONCAT, FIRST_FRAME = 1, 2      # fyc.h FYC_FIRST_*: bits of build_unet_input_first's mode
+
+
+def build_unet_input_first(latents, first, dup, dtype, mode, c_pad=None, out=None):
+    """Step prologue of the first-frame-conditioned models (fyc.h fyc_build_unet_input_first): latents (b,4,f,h,w) fp32, first (b,4,h,w)
+    fp32 -> [dup*b, f, h, w, 8 | 4].  ``mode`` & FIRST_CONCAT: [latents | first on every frame]; ``mode`` & FIRST_FRAME: frame 0 of
+    ``latents`` is overwritten with ``first`` in place first (the caller's persistent latents, read by the DDIM step that follows)."""
+    assert latents.dtype == torch.float32 and latents.is_contiguous() and latents.is_cuda
+    b, c, f, h, w = latents.shape
+    assert c == 4 and first is not None and first.dtype == torch.float32 and first.is_contiguous() and tuple(first.shape) == (b, 4, h, w)
+    assert mode in (FIRST_CONCAT, FIRST_FRAME, FIRST_CONCAT | FIRST_FRAME)
+    cin = 8 if mode & FIRST_CONCAT else 4
+    c_pad = cin if c_pad is None else c_pad
+    if out is None:
+        out = torch.empty((dup * b, f, h, w, c_pad), dtype=dtype, device=latents.device)
+    assert out.shape == (dup * b, f, h, w, c_pad) and out.dtype == dtype and out.is_contiguous()
+    check(lib().fyc_build_unet_input_first(ptr(latents), ptr(first), ptr(out), b, f, h * w, dup, mode, c_pad, dtype_code(dtype), stream_ptr()))
+    return out
+
+
+def first_frame_temb_rows(temb, B, F):
+    """temb [B + 1, N] fp32 (t = 0 row last) -> [B * F, N]: row b F + f = temb[B] for f == 0, else temb[b] (fyc.h
+    fyc_first_frame_temb_rows; the per-image row bias of every conv1 under use_first_frame_condition)."""
+    assert temb.dtype == torch.float32 and temb.is_contiguous() and temb.is_cuda and temb.shape[0] == B + 1
+    N = temb.shape[1]
+    out = torch.empty((B * F, N), dtype=torch.float32, device=temb.device)
+    check(lib().fyc_first_frame_temb_rows(ptr(temb), ptr(out), B, F, N, stream_ptr()))
+    return out
+
+
 def cfg_ddim_step(pred, sample, coefs, noise=None, out=None, single=None, video_scale=0.0):
     """pred fp32 [2, ...] (uncond, cond) if coefs.cfg_pair else [1, ...]; sample fp32; returns prev sample.
     ``single`` (same shape as sample): the per-frame prediction of the video_scale > 0 branch (pipeline_animation.py:738-761)."""

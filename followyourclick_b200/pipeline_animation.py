@@ -131,6 +131,32 @@ def prepare_first_frame_condition(vae, first_images, first_images_mask, generato
     return lat, torch.clamp(mask, 0, 1)
 
 
+def check_first_frame_options(use_first_frame_condition=False, use_first_frame_condition_concat=False,
+                              use_first_frame_mask_condition_concat=False, first_image_latents=None, video_scale=0, unet_batch=1,
+                              use_fps_condition=False, use_camera_motion_condition=False):
+    """The combinations of the two first-frame condition modes with the other options that the reference pipeline cannot sample
+    (pipeline_animation.py:686-773 with unet.py:422-590 and resnet.py:304-320) raise here, each with a message naming both options;
+    every other combination is sampled.  ``unet_batch``: rows of the UNet's batch (2 b under classifier-free guidance)."""
+    modes = [n for n, on in (("use_first_frame_condition", use_first_frame_condition),
+                             ("use_first_frame_condition_concat", use_first_frame_condition_concat)) if on]
+    for m in modes:
+        if first_image_latents is None:
+            raise ValueError(f"{m} needs first_image_latents (the clean first-image latents, (b, 4, h, w))")
+        if use_first_frame_mask_condition_concat:
+            raise ValueError(f"{m} with use_first_frame_mask_condition_concat: the reference has no UNet input for the pair "
+                             "(pipeline_animation.py:691-705 builds the mask-concat input only without use_first_frame_condition; "
+                             "with use_first_frame_condition_concat conv_in would get 13 channels)")
+    if use_first_frame_condition_concat and video_scale > 0:
+        raise ValueError("use_first_frame_condition_concat with video_scale > 0: the reference's per-frame forward passes the 4-channel latents "
+                         "without the first-image concat (pipeline_animation.py:738-751), which the 8-channel conv_in rejects")
+    if use_first_frame_condition and unet_batch > 1:
+        for other, on in (("use_fps_condition", use_fps_condition), ("use_camera_motion_condition", use_camera_motion_condition)):
+            if on:
+                raise ValueError(f"use_first_frame_condition with {other} at a UNet batch of {unet_batch} (classifier-free guidance doubles it): "
+                                 f"the reference adds the {unet_batch}-row {other} embedding to the {unet_batch + 1}-row time embedding of the "
+                                 "first-frame condition (unet.py:523-558), which broadcasts only for a batch of 1")
+
+
 class AnimationPipeline:
     _optional_components = []
     use_cuda_graph = True          # replay one captured UNet forward per DDIM step (set False to launch kernel by kernel)
@@ -282,16 +308,23 @@ class AnimationPipeline:
                 first_images_mask=None, use_first_frame_mask_condition_concat=False, fps_tensor=None, flow_control=None,
                 use_fps_condition=False, use_ip_cross_attention=False, image_clip_feat_pair=None,
                 use_camera_motion_condition=False, camera_movement_type=None, eta=0.0, generator=None, callback=None,
-                callback_steps=1, progress=False, video_scale=0):
+                callback_steps=1, progress=False, video_scale=0, use_first_frame_condition=False,
+                use_first_frame_condition_concat=False):
         """pipeline_animation.py:686-773 on the engine.  latents fp32 (b,4,F,h,w) on device; returns final latents.
         video_scale > 0 (:738-761): a second forward per step on the clip's frames taken one at a time, combined as
-        ``s + video_scale (u - s) + guidance (c - u)`` (SURVEY 8f row 3)."""
+        ``s + video_scale (u - s) + guidance (c - u)`` (SURVEY 8f row 3).
+        use_first_frame_condition (:691-692): frame 0 of the latents is replaced by ``first_image_latents`` before every step, so the
+        step reads the replaced frame (the last step's output is not replaced); use_first_frame_condition_concat (:717-719): the UNet
+        input is [latents | first_image_latents on every frame].  Both go through one prologue kernel (ops.build_unet_input_first)."""
         dev = self.unet.device
         do_cfg = guidance_scale > 1.0
         if video_scale > 0 and not do_cfg:
             raise NotImplementedError("video_scale > 0 without classifier-free guidance (the reference only uses the per-frame "
                                       "prediction inside its CFG combine, pipeline_animation.py:757-761)")
         dup = 2 if do_cfg else 1
+        check_first_frame_options(use_first_frame_condition, use_first_frame_condition_concat, use_first_frame_mask_condition_concat,
+                                  first_image_latents, video_scale, dup * latents.shape[0], use_fps_condition, use_camera_motion_condition)
+        mode = (ops.FIRST_CONCAT if use_first_frame_condition_concat else 0) | (ops.FIRST_FRAME if use_first_frame_condition else 0)
         sched, unet = self.scheduler, self.unet
         sched.set_timesteps(num_inference_steps, device=dev)
         t_host = list(sched._timesteps_host)
@@ -310,11 +343,25 @@ class AnimationPipeline:
             if first_images_mask is not None:
                 mask = first_images_mask[:, :, 0].to(device=dev, dtype=torch.float32).contiguous()     # :632-635 (frame 0, clamp in-kernel)
         latents = latents.to(device=dev, dtype=torch.float32).contiguous()
+        ff_first = None
+        if mode:
+            ff_first = first_image_latents.to(device=dev, dtype=torch.float32).contiguous()
+            if mode & ops.FIRST_FRAME:
+                latents = latents.clone()      # the prologue writes frame 0 in place: never into the caller's tensor
         text_embeddings = text_embeddings.to(dev)
         c_pad = unet.input_channel_pad() if hasattr(unet, "input_channel_pad") else None
         bar = self.progress_bar(total=num_inference_steps) if progress else _NullBar()
         flags = dict(use_ip_cross_attention=use_ip_cross_attention, use_camera_motion_condition=use_camera_motion_condition,
                      use_fps_condition=use_fps_condition)
+        if mode & ops.FIRST_CONCAT:
+            flags["use_first_frame_condition_concat"] = True
+        if mode & ops.FIRST_FRAME:
+            flags["use_first_frame_condition"] = True
+
+        def prologue(out=None):
+            if mode:
+                return ops.build_unet_input_first(latents, ff_first, xdup, unet.dtype, mode, c_pad=c_pad, out=out)
+            return ops.build_unet_input(latents, mask, first, xdup, unet.dtype, c_pad=c_pad, out=out)
         clip_d = None if image_clip_feat_pair is None else image_clip_feat_pair.to(dev)
         graphed = context = graphed_sf = context_sf = None
         b, _, f, h, w = latents.shape
@@ -328,12 +375,12 @@ class AnimationPipeline:
         share = 2 if (self.share_cfg_prefix and do_cfg and hasattr(unet, "prepare_context")) else 1
         xdup = dup // share
         if self.use_cuda_graph and hasattr(unet, "forward_nfhwc"):
-            cin = c_pad if c_pad is not None else (9 if first is not None else 4)
+            cin = c_pad if c_pad is not None else (9 if first is not None else 8 if mode & ops.FIRST_CONCAT else 4)
             # everything the captured forward's control flow depends on: shapes, dtype, flags, WHICH optional inputs exist, and the
             # IP-attention logit-scale semantics (enable_xformers_memory_efficient_attention toggles it without re-packing weights)
             key = (xdup * b, share, self.hoist_context, f, h, w, cin, unet.dtype, tuple(sorted(flags.items())), tuple(text_embeddings.shape),
                    None if clip_d is None else tuple(clip_d.shape), fps_d is None, flow_d is None, cam_d is None,
-                   bool(getattr(unet, "_xformers_semantics", False)))
+                   bool(getattr(unet, "_xformers_semantics", False)), mode)
             cache = self.__dict__.setdefault("_graph_cache", OrderedDict())
             graphed = cache.get(key)
             if graphed is not None:
@@ -354,7 +401,7 @@ class AnimationPipeline:
         with bar as pb:
             for i, t in enumerate(t_host):
                 if graphed is not None:
-                    ops.build_unet_input(latents, mask, first, xdup, unet.dtype, c_pad=c_pad, out=graphed.x)
+                    prologue(out=graphed.x)
                     graphed.t.copy_(t_dev[i])
                     graphed.replay()
                     pred = graphed.pred
@@ -365,7 +412,7 @@ class AnimationPipeline:
                 else:
                     if i == 0 and self.hoist_context and hasattr(unet, "prepare_context"):
                         context = unet.prepare_context(text_embeddings, clip_d, use_ip_cross_attention)
-                    x = ops.build_unet_input(latents, mask, first, xdup, unet.dtype, c_pad=c_pad)
+                    x = prologue()
                     y = unet.forward_nfhwc(x, t_dev[i], text_embeddings, fps_tensor=fps_d, flow_control=flow_d,
                                            reference_images_clip_feat=clip_d, camera_movement_type_tensor=cam_d, context=context,
                                            **(dict(flags, cfg_dup=share) if share > 1 else flags))
@@ -392,8 +439,7 @@ class AnimationPipeline:
                  use_uncond_images=False, use_camera_motion_condition=False, camera_movement_type=None,
                  use_text_encoder_2=False, use_uncond_text_2=False, use_fps_condition=False, fps_tensor=None,
                  use_interpolate_noise=False, first_images_mask=None, flow_control=None, **kwargs):
-        if use_first_frame_condition or use_first_frame_condition_concat or use_text_encoder_2 or use_first_image_as_init_latents \
-                or use_first_frame_mask_condition_concat_image_partial_mask is not None:
+        if use_text_encoder_2 or use_first_image_as_init_latents or use_first_frame_mask_condition_concat_image_partial_mask is not None:
             raise NotImplementedError("option outside the scripts/inference.py path (SURVEY 8f)")
         height = height or self.unet.config.sample_size * self.vae_scale_factor
         width = width or self.unet.config.sample_size * self.vae_scale_factor
@@ -405,6 +451,9 @@ class AnimationPipeline:
             batch_size = len(prompt)
         device = self._execution_device
         do_cfg = guidance_scale > 1.0
+        check_first_frame_options(use_first_frame_condition, use_first_frame_condition_concat, use_first_frame_mask_condition_concat,
+                                  first_image_latents, video_scale, (2 if do_cfg else 1) * batch_size * num_videos_per_prompt,
+                                  use_fps_condition, use_camera_motion_condition)
         prompt = prompt if isinstance(prompt, list) else [prompt] * batch_size
         if negative_prompt is not None:
             negative_prompt = negative_prompt if isinstance(negative_prompt, list) else [negative_prompt] * batch_size
@@ -424,7 +473,9 @@ class AnimationPipeline:
                                use_ip_cross_attention=use_ip_cross_attention, image_clip_feat_pair=clip_pair,
                                use_camera_motion_condition=use_camera_motion_condition, camera_movement_type=camera_movement_type,
                                eta=eta, generator=generator if not isinstance(generator, list) else None,
-                               callback=callback, callback_steps=callback_steps, progress=self._progress, video_scale=video_scale)
+                               callback=callback, callback_steps=callback_steps, progress=self._progress, video_scale=video_scale,
+                               use_first_frame_condition=use_first_frame_condition,
+                               use_first_frame_condition_concat=use_first_frame_condition_concat)
         video = self.decode_latents(latents)
         if output_type == "tensor":
             video = torch.from_numpy(video)

@@ -437,8 +437,10 @@ class UNet3DConditionModel(ParamTreeModel):
             return w, b, offs
         return self._cached(("temb_pack",), make)
 
-    def _resnet(self, p, x, temb_all, B, F, skip=None):
-        """``skip``: the up blocks' `torch.cat([hidden_states, res_hidden_states], dim=1)` (unet_blocks.py:763,885) is not materialised -
+    def _resnet(self, p, x, temb_all, B, F, skip=None, temb_per_image=False):
+        """``temb_per_image``: ``temb_all`` holds one row per image (use_first_frame_condition, ops.first_frame_temb_rows) instead of one
+        per clip.
+        ``skip``: the up blocks' `torch.cat([hidden_states, res_hidden_states], dim=1)` (unet_blocks.py:763,885) is not materialised -
         norm1 normalises [x | skip] reading both tensors in place, the 1x1 shortcut runs its K loop over the two sources.  A skip with
         fewer images than x (the conv_in output under the shared CFG prefix: ONE copy for the `rep` CFG replicas of x) is read once per
         replica instead of being duplicated."""
@@ -455,7 +457,8 @@ class UNet3DConditionModel(ParamTreeModel):
                 ops.groupnorm(x[r * nb:(r + 1) * nb], self._f(p + ".norm1.weight"), self._f(p + ".norm1.bias"), self._cfg["norm_num_groups"],
                               self._cfg["norm_eps"], silu=True, stat_batches=nb if self._cfg["use_inflated_groupnorm"] else B // rep,
                               x2=skip, out=h[r * nb:(r + 1) * nb])
-        h = ops.conv3x3(h, self._conv_w(p + ".conv1.weight"), bias=self._f(p + ".conv1.bias"), rowbias=temb, images_per_group=F)
+        h = ops.conv3x3(h, self._conv_w(p + ".conv1.weight"), bias=self._f(p + ".conv1.bias"), rowbias=temb,
+                        images_per_group=1 if temb_per_image else F)
         h = self._gn(p + ".norm2", h, B, True, False)
         if self._has(p + ".conv_shortcut.weight"):
             w_s, b_s = self._w1x1(p + ".conv_shortcut.weight"), self._f(p + ".conv_shortcut.bias")
@@ -575,10 +578,13 @@ class UNet3DConditionModel(ParamTreeModel):
         return out.view(NB, H, W, C)
 
     # ------------------------------------------------------------------------------------------ forward
-    def _embed(self, name, values, B, residual=None):
+    def _embed(self, name, values, B, residual=None, zero_row=False):
+        """``zero_row``: a timestep 0 is appended after the B rows (use_first_frame_condition, unet.py:523-524)."""
         dev = self.device
         v = torch.as_tensor(values)
         v = (v.reshape(1) if v.dim() == 0 else v.reshape(-1)).to(device=dev, dtype=torch.int64).expand(B).contiguous()
+        if zero_row:
+            v = torch.cat([v, torch.zeros(1, dtype=torch.int64, device=dev)])
         s = ops.timestep_embed(v, self._freqs(), self._cfg["flip_sin_to_cos"])
         h = ops.silu(ops.gemm(s, self._fw(name + ".linear_1.weight"), bias=self._f(name + ".linear_1.bias")))
         return ops.gemm(h, self._fw(name + ".linear_2.weight"), bias=self._f(name + ".linear_2.bias"), residual=residual)
@@ -685,7 +691,7 @@ class UNet3DConditionModel(ParamTreeModel):
     def forward_nfhwc(self, x, timestep, encoder_hidden_states, fps_tensor=None, flow_control=None,
                       reference_images_clip_feat=None, camera_movement_type_tensor=None, use_ip_cross_attention=False,
                       use_camera_motion_condition=False, use_fps_condition=False, use_first_frame_condition_concat=False,
-                      context=None, cfg_dup=1):
+                      context=None, cfg_dup=1, use_first_frame_condition=False):
         """Engine entry: x [B, F, H, W, Cin] channels-last in the compute dtype -> fp32 [B, F, H, W, out_channels] (possibly a
         [..., :out_channels] view of a wider buffer; ops.nfhwc_to_ncfhw takes it as is).  ``context``: a ClipContext from
         ``prepare_context`` - then encoder_hidden_states / reference_images_clip_feat are not read (hoisted out of the loop).
@@ -693,7 +699,9 @@ class UNet3DConditionModel(ParamTreeModel):
         hold the CFG pair (2b rows, [uncond..., cond...]).  The reference feeds ``torch.cat([latents] * 2)`` (pipeline_animation.py:
         709), so until the first cross-attention reads the text context both halves of its batch carry identical values: conv_in, the
         first ResnetBlock3D and the first transformer's GroupNorm, proj_in, self-attention (the most expensive attention of the
-        network) and query projection are computed once here and fan out at that cross-attention.  Output: [2b, F, H, W, out]."""
+        network) and query projection are computed once here and fan out at that cross-attention.  Output: [2b, F, H, W, out].
+        ``use_first_frame_condition`` (unet.py:523-524, resnet.py:304-320): frame 0 of every clip gets the time embedding of t = 0, the
+        other frames their clip's."""
         ops.require_cuda(x, "UNet3DConditionModel")
         cfg = self._cfg
         B, F, H, W, Cin = x.shape
@@ -704,15 +712,25 @@ class UNet3DConditionModel(ParamTreeModel):
         if dup > 1 and not (n > 1 and cfg["layers_per_block"] >= 1):
             raise ValueError("cfg_dup needs a cross-attention block at the first level")
         B = B * dup                       # batch of everything from the first cross-attention on (and of the embeddings)
-        emb = self._embed("time_embedding", timestep, B)
-        if use_camera_motion_condition:
-            emb = self._embed("camera_motion_embedding", camera_movement_type_tensor, B, residual=emb)
+        ff = bool(use_first_frame_condition)
+        if ff and B > 1 and (use_camera_motion_condition or use_fps_condition):
+            # unet.py:523-558: the reference adds a B-row camera / fps / motion embedding to the (B + 1)-row emb of the first-frame
+            # condition, which only broadcasts for B == 1
+            raise ValueError(f"use_first_frame_condition with {'use_camera_motion_condition' if use_camera_motion_condition else 'use_fps_condition'}"
+                             f" needs a UNet batch of 1 (got {B}): the reference adds the {B}-row condition embedding to the {B + 1}-row time "
+                             "embedding of the first-frame condition, which does not broadcast")
+        ne = B + 1 if ff else B           # rows of emb: the first-frame condition appends the t = 0 row (unet.py:523-524)
+        emb = self._embed("time_embedding", timestep, B, zero_row=ff)
+        if use_camera_motion_condition:   # (ne = 2 rows of one value when ff: the reference's broadcast of its 1-row embedding)
+            emb = self._embed("camera_motion_embedding", camera_movement_type_tensor, ne, residual=emb)
         if use_fps_condition:
-            emb = self._embed("fps_embedding", fps_tensor, B, residual=emb)
-            emb = self._embed("motion_embedding", flow_control, B, residual=emb)
+            emb = self._embed("fps_embedding", fps_tensor, ne, residual=emb)
+            emb = self._embed("motion_embedding", flow_control, ne, residual=emb)
         semb = ops.silu(emb)                                     # every resnet applies SiLU to emb first (resnet.py:307)
         tw, tb, _ = self._temb_pack()
         semb = ops.gemm(semb, tw, bias=tb)                       # [B, sum Cout]: all 22 time_emb_proj at once (see _temb_pack)
+        if ff:                                                   # [B F, sum Cout]: frame 0 of each clip -> the t = 0 row (resnet.py:304-320)
+            semb = ops.first_frame_temb_rows(semb, B, F)
         # step-invariant conditioning: built here when the caller has not hoisted it out of the DDIM loop (``context``)
         ctx = context if context is not None else self.prepare_context(
             encoder_hidden_states, reference_images_clip_feat, use_ip_cross_attention)
@@ -742,7 +760,7 @@ class UNet3DConditionModel(ParamTreeModel):
         for i in range(n):
             p = f"down_blocks.{i}"
             for j in range(cfg["layers_per_block"]):
-                x = self._resnet(f"{p}.resnets.{j}", x, semb, B // dup if shared else B, F)
+                x = self._resnet(f"{p}.resnets.{j}", x, semb, B // dup if shared else B, F, temb_per_image=ff)
                 if i < n - 1:
                     x = self._transformer(f"{p}.attentions.{j}", x, ctx, self._heads[i], F, dup=dup if shared else 1)
                     shared = False
@@ -753,18 +771,18 @@ class UNet3DConditionModel(ParamTreeModel):
                 x = ops.conv3x3(x, self._conv_w(f"{p}.downsamplers.0.conv.weight"), bias=self._f(f"{p}.downsamplers.0.conv.bias"), stride=2)
                 skips.append(x)
             self._tap(f"down{i}", x)
-        x = self._resnet("mid_block.resnets.0", x, semb, B, F)
+        x = self._resnet("mid_block.resnets.0", x, semb, B, F, temb_per_image=ff)
         x = self._transformer("mid_block.attentions.0", x, ctx, self._heads[-1], F)
         if cfg["use_motion_module"] and cfg["motion_module_mid_block"]:
             x = self._motion("mid_block.motion_modules.0", x, B, F)
-        x = self._resnet("mid_block.resnets.1", x, semb, B, F)
+        x = self._resnet("mid_block.resnets.1", x, semb, B, F, temb_per_image=ff)
         self._tap("mid", x)
         for i in range(n):
             p = f"up_blocks.{i}"
             lvl = n - 1 - i
             for j in range(cfg["layers_per_block"] + 1):
                 skip = skips.pop()                       # (under the shared CFG prefix the conv_in output exists once: _resnet reads it per replica)
-                x = self._resnet(f"{p}.resnets.{j}", x, semb, B, F, skip=skip)
+                x = self._resnet(f"{p}.resnets.{j}", x, semb, B, F, skip=skip, temb_per_image=ff)
                 if i > 0:
                     x = self._transformer(f"{p}.attentions.{j}", x, ctx, self._heads[lvl], F)
                 if motion_on(lvl, True):
@@ -787,7 +805,7 @@ class UNet3DConditionModel(ParamTreeModel):
                 encoder_hidden_states_2=None, use_fps_condition=False, fps_tensor=None, first_images_mask=None,
                 flow_control=None):
         """Same signature/semantics as animatediff/models/unet.py:422-672 (sample: (b, c, f, h, w))."""
-        if use_first_frame_condition or use_text_encoder_2 or class_labels is not None or attention_mask is not None:
+        if use_text_encoder_2 or class_labels is not None or attention_mask is not None:
             raise NotImplementedError("forward option outside the shipped inference path")
         x = sample.to(device=self.device, dtype=torch.float32)
         if use_first_frame_condition_concat and reference_images_latent is not None:          # unet.py:578-583
@@ -800,7 +818,8 @@ class UNet3DConditionModel(ParamTreeModel):
                                use_ip_cross_attention=use_ip_cross_attention,
                                use_camera_motion_condition=use_camera_motion_condition,
                                use_fps_condition=use_fps_condition,
-                               use_first_frame_condition_concat=use_first_frame_condition_concat)
+                               use_first_frame_condition_concat=use_first_frame_condition_concat,
+                               use_first_frame_condition=use_first_frame_condition)
         out = ops.nfhwc_to_ncfhw(y)
         if not return_dict:
             return (out,)

@@ -256,6 +256,23 @@ int32_t fyc_nfhwc_to_ncfhw(const void* in, float* out, int64_t B, int64_t C, int
  * written as zeros (lets the 9-channel stem run on the tensor-core path with a 16-channel, zero-extended filter). */
 int32_t fyc_build_unet_input(const float* latents, const float* mask, const float* first, void* out, int64_t b,
                              int64_t F, int64_t HW, int32_t dup, int32_t c_pad, int32_t dtype, void* stream);
+/* The same step prologue for the first-frame-conditioned motion models; `mode` is a bit set, first (b,4,H,W) fp32 the clean first-image
+ * latents:
+ *   FYC_FIRST_CONCAT (use_first_frame_condition_concat): out = [latents(4) | first(4) on every frame], Cin = 8.  Replaces the CFG
+ *       duplication `torch.cat([latents] * 2)` (pipeline_animation.py:709) followed by the UNet's own concat of the duplicated
+ *       first-image latents repeated over the frames (`torch.cat([first_image_latents] * 2)`, :717-719; unet.py:578-583);
+ *   FYC_FIRST_FRAME (use_first_frame_condition): frame 0 of `latents` is overwritten IN PLACE with `first`, then out = latents, Cin = 4.
+ *       Replaces `latents[:, :, 0, :, :] = first_image_latents` (pipeline_animation.py:691-692), which writes the tensor the DDIM step
+ *       of the same iteration reads as its sample: the caller passes its persistent latents.
+ * Both bits together do both (the reference runs that combination too).  Channels Cin..c_pad-1 are written as zeros. */
+enum { FYC_FIRST_CONCAT = 1, FYC_FIRST_FRAME = 2 };
+int32_t fyc_build_unet_input_first(float* latents, const float* first, void* out, int64_t b, int64_t F, int64_t HW, int32_t dup,
+                                   int32_t mode, int32_t c_pad, int32_t dtype, void* stream);
+/* Time-embedding row table of use_first_frame_condition (unet.py:523-524 appends a zero timestep, so emb has B + 1 rows; resnet.py:304-320
+ * adds row B to frame 0 of every clip and row b to frames 1.. of clip b): temb [B + 1, N] fp32 (the fused time_emb_proj GEMV of all
+ * ResnetBlock3Ds, t = 0 row last) -> out [B * F, N], out[b F + f] = temb[f == 0 ? B : b].  conv1 reads it as its row bias with
+ * images_per_group = 1. */
+int32_t fyc_first_frame_temb_rows(const float* temb, float* out, int64_t B, int64_t F, int64_t N, void* stream);
 /* CFG combine + DDIMScheduler.step (pipeline_animation.py:763-764 + scheduling_ddim.py:308-349), fp32, exact
  * reference operation order (no FMA contraction).  pred: [2, n] (uncond, cond) when c->cfg_pair else [1, n]. */
 typedef struct {
