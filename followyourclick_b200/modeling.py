@@ -186,7 +186,7 @@ class ParamTreeModel(nn.Module):
 
     def _conv_w_up2(self, key):
         """phase-summed filter of an upsampler conv, [4, Cout, 2, 2, Cin] (16-bit tensor-core mode only, else None)"""
-        if self._compute_dtype not in (torch.bfloat16, torch.float16):
+        if self._compute_dtype not in ops.HALF_DTYPES:
             return None
         return self._cached(("up2", key), lambda: upsample_phase_weights(self._p(key).detach().float()).to(self._compute_dtype).contiguous())
 
@@ -194,7 +194,6 @@ class ParamTreeModel(nn.Module):
         """(filter [N, 3, 3, Cin], bias [N], true Cout) of a 3- / 4-channel output convolution.  In tensor-core mode the output
         channels are zero-padded to N = 16 so the head is a tensor-core implicit GEMM (its N must be a multiple of 16) instead of a
         CUDA-core kernel; consumers read the first Cout of the 16 channels (fyc_nfhwc_to_ncfhw / fyc_frames_finalize `ldc`)."""
-        from . import ops
         cout = self._p(name + ".weight").shape[0]
         if not (ops.use_tc_head and cout < 16 and ops.tc_ok(self._compute_dtype, pixels)):
             return self._conv_w(name + ".weight"), self._f(name + ".bias"), cout

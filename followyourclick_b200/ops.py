@@ -13,7 +13,6 @@ from . import _lib as L
 from ._lib import check, dtype_code, lib, ptr, stream_ptr
 
 _impl = L.IMPL_AUTO
-L_SIMT = L.IMPL_SIMT
 _prof_shapes = False   # per-shape family names in the profile (diagnostics)
 _prof = None      # list of (family, algorithmic_flops, algorithmic_bytes, start_event, end_event) while profiling
 _pad_flops = 0.0  # FLOPs of the last profile that multiplied zero padding (q/k heads 40 -> 64, 9 -> 16 channel stem, 4 -> 16 channel head)
@@ -109,16 +108,28 @@ def check_compute_dtype(dtype):
         raise ValueError(f"unsupported compute dtype {dtype}: expected torch.float32, torch.bfloat16 or torch.float16")
 
 
-def tc_ok(dtype, M):
-    return _impl != L.IMPL_SIMT and dtype in HALF_DTYPES and M >= 64 and lib().fyc_tcgen05_available() == 1
+def tc_available():
+    """does this device run the tensor-core kernels?  The one hardware query under every route rule below (the CPU tests' kernel
+    emulator answers it with True and keeps the rules themselves)."""
+    return lib().fyc_tcgen05_available() == 1
+
+
+def _tc_open(dtype, impl):
+    """the tensor-core routes are open to a call: 16-bit operands, neither the global setting nor the call's ``impl`` is IMPL_SIMT,
+    and the device runs the tensor-core kernels"""
+    return _impl != L.IMPL_SIMT and impl != L.IMPL_SIMT and dtype in HALF_DTYPES and tc_available()
+
+
+def tc_ok(dtype, M, impl=None):
+    return M >= 64 and _tc_open(dtype, impl)
 
 
 use_ln_fold = os.environ.get("FYC_LN_FOLD", "1") != "0"          # A/B switch: LayerNorm folded into the consuming GEMM's epilogue
 
 
-def ln_fold_ok(dtype, M, C):
+def ln_fold_ok(dtype, M, C, impl=None):
     """can a LayerNorm over C channels feeding a GEMM on M rows be folded into that GEMM (fyc.h FYC_EPI_LNFOLD: tensor-core path only)?"""
-    return use_ln_fold and tc_ok(dtype, M) and C % 8 == 0 and C <= 2048
+    return use_ln_fold and C % 8 == 0 and C <= 2048 and tc_ok(dtype, M, impl)
 
 
 def layernorm_stats(x, eps=1e-5):
@@ -185,18 +196,18 @@ def gemm(A, W, bias=None, residual=None, rowbias=None, rows_per_group=0, alpha=1
     ``A2`` [M, K2]: the K dimension is the concatenation [A | A2] read in place."""
     _cuda(A, "gemm.A"); _cuda(W, "gemm.W"); _cuda(residual, "gemm.residual"); _cuda(A2, "gemm.A2")
     _f32vec(bias, "gemm.bias"); _f32vec(rowbias, "gemm.rowbias")
+    impl = _impl if impl is None else impl
     K1 = 0
     if A2 is not None:
         # A = [A | A2] along K without the concatenation ever being written (fyc.h A2): tensor-core path with K1 % 64 == 0, else concatenate
         assert A.dim() == 2 and A2.dim() == 2 and A2.shape[0] == A.shape[0] and A2.dtype == A.dtype
-        if (_impl if impl is None else impl) != L.IMPL_SIMT and tc_ok(A.dtype, A.shape[0]) and A.shape[1] % 64 == 0 and A2.shape[1] % 8 == 0 and use_dual_source:
+        if tc_ok(A.dtype, A.shape[0], impl) and A.shape[1] % 64 == 0 and A2.shape[1] % 8 == 0 and use_dual_source:
             K1 = A.shape[1]
         else:
             A, A2 = concat_channels(A.contiguous(), A2.contiguous()), None
     if ln is not None:
         _f32vec(ln, "gemm.ln_rstd")
         assert A2 is None and A.dim() == 2 and ln.shape == (A.shape[0],)
-    impl = _impl if impl is None else impl
     batched = A.dim() == 3
     if batched:
         Bn, M, K = A.shape
@@ -209,7 +220,7 @@ def gemm(A, W, bias=None, residual=None, rowbias=None, rows_per_group=0, alpha=1
     if K1:
         K = K1 + A2.shape[1]
     assert W.shape[-1] == K and W.dtype == A.dtype
-    fused_geglu = geglu and impl != L.IMPL_SIMT and tc_ok(A.dtype, M)
+    fused_geglu = geglu and tc_ok(A.dtype, M, impl)
     n_out = N // 2 if fused_geglu else N
     if geglu and not fused_geglu and out is not None and not out.is_contiguous():
         # fyc_geglu writes packed [M, N / 2] rows: a wider row stride would put rows in the wrong place and write outside the view
@@ -227,7 +238,7 @@ def gemm(A, W, bias=None, residual=None, rowbias=None, rows_per_group=0, alpha=1
                    o.stride(-2), residual.stride(-2) if residual is not None else 0, Bn, sA, sW,
                    o.stride(0) if batched else 0, rows_per_group, float(alpha), dtype_code(A.dtype), epi, impl,
                    ptr(A2) if K1 else None, A2.stride(0) if K1 else 0, K1, ptr(ln))
-    fam = "gemm_tc" if (impl != L.IMPL_SIMT and tc_ok(A.dtype, M) and N % 16 == 0 and K % 8 == 0) else "gemm_simt"
+    fam = "gemm_tc" if (tc_ok(A.dtype, M, impl) and N % 16 == 0 and K % 8 == 0) else "gemm_simt"
     if _prof_shapes:
         fam += f"[{Bn}x{M}x{N}x{K}{'g' if fused_geglu else ''}{'r' if residual is not None else ''}{'L' if ln is not None else ''}]"
     with _rec(fam, 2.0 * Bn * M * N * K, A.element_size() * Bn * (M * K + N * K + M * n_out)):
@@ -242,6 +253,13 @@ def gemm(A, W, bias=None, residual=None, rowbias=None, rows_per_group=0, alpha=1
 
 use_up2_phases = os.environ.get("FYC_UP2_PHASES", "1") != "0"    # A/B switch for the four-phase upsample convolution
 use_tc_head = os.environ.get("FYC_TC_HEAD", "1") != "0"          # A/B switch: 3- / 4-channel output convs zero-padded to N = 16 on the tensor cores
+
+
+def up2_phases_ok(dtype, pixels, residual, rowbias, out_f32, impl=None):
+    """the host side of the four-phase upsampler route for a conv over ``pixels`` low-res pixels (``residual`` / ``rowbias``: the call's
+    operands or None): a bias-only epilogue with a 16-bit output on the tensor cores.  The C query fyc_conv3x3_up2_eligible decides
+    the rest (the patch geometry)."""
+    return use_up2_phases and residual is None and rowbias is None and not out_f32 and tc_ok(dtype, pixels, impl)
 
 
 def conv3x3(x, w, bias=None, residual=None, rowbias=None, images_per_group=0, stride=1, upsample=1, out_f32=False, impl=None,
@@ -261,8 +279,7 @@ def conv3x3(x, w, bias=None, residual=None, rowbias=None, images_per_group=0, st
     impl = _impl if impl is None else impl
     NB, H, W_, Cin = x.shape
     Cout = w.shape[0]
-    if upsample == 2 and w_phases is not None and use_up2_phases and impl != L.IMPL_SIMT and tc_ok(x.dtype, NB * H * W_) \
-            and residual is None and rowbias is None and not out_f32:
+    if upsample == 2 and w_phases is not None and up2_phases_ok(x.dtype, NB * H * W_, residual, rowbias, out_f32, impl):
         assert w_phases.is_contiguous() and w_phases.dtype == x.dtype and tuple(w_phases.shape) == (4, Cout, 2, 2, Cin)
         out = torch.empty((NB, 2 * H, 2 * W_, Cout), dtype=x.dtype, device=x.device)
         a = L.ConvArgs(ptr(x), ptr(w), ptr(out), ptr(bias), None, None, NB, H, W_, Cin, Cout, 1, 2, 0, dtype_code(x.dtype),
@@ -273,7 +290,7 @@ def conv3x3(x, w, bias=None, residual=None, rowbias=None, images_per_group=0, st
             with _rec(fam, 2.0 * NB * H * W_ * Cout * 16 * Cin, x.element_size() * (x.numel() + w_phases.numel() + out.numel())):
                 check(lib().fyc_conv3x3(C.byref(a), stream_ptr()))
             return out
-    if upsample == 2 and impl != L.IMPL_SIMT and tc_ok(x.dtype, NB * H * W_):
+    if upsample == 2 and tc_ok(x.dtype, NB * H * W_, impl):
         x = upsample_nearest2x(x)            # the tensor-core path reads unit-stride boxes: materialise the upsample
         NB, H, W_, Cin = x.shape
         upsample = 1
@@ -388,8 +405,8 @@ def _tc_entry(name, t):
     return getattr(lib(), name + "_f16" if t.dtype == torch.float16 else name)
 
 
-def self_attention_tc_ok(dtype, L, D):
-    return _impl != L_SIMT and dtype in HALF_DTYPES and D in (40, 64) and L % 128 == 0 and lib().fyc_tcgen05_available() == 1
+def self_attention_tc_ok(dtype, L, D, impl=None):
+    return D in (40, 64) and L % 128 == 0 and _tc_open(dtype, impl)
 
 
 def self_attention_tc(qk, q_col0, k_col0, vt, heads, D, scale):
@@ -406,8 +423,8 @@ def self_attention_tc(qk, q_col0, k_col0, vt, heads, D, scale):
 use_attn_d80 = os.environ.get("FYC_ATTN_D80", "1") != "0"        # A/B switch: head-dim-80 self-attention on the wgmma kernel (else the mma.sync kernel)
 
 
-def self_attention_tc80_ok(dtype, L, D):
-    return use_attn_d80 and _impl != L_SIMT and dtype in HALF_DTYPES and D == 80 and L % 256 == 0 and lib().fyc_tcgen05_available() == 1
+def self_attention_tc80_ok(dtype, L, D, impl=None):
+    return use_attn_d80 and D == 80 and L % 256 == 0 and _tc_open(dtype, impl)
 
 
 def self_attention_tc_d80(qkv, q_col0, k_col0, vt, heads, scale):
@@ -426,9 +443,8 @@ use_cross_tc = os.environ.get("FYC_CROSS_TC", "1") != "0"        # A/B switch: t
 CROSS_LK, CROSS_LK2 = 80, 16                                      # padded key counts of the resident-context kernel
 
 
-def cross_attention_tc_ok(dtype, D, Lk, Lk2):
-    return (use_cross_tc and _impl != L_SIMT and dtype in HALF_DTYPES and D in (40, 64, 80) and 1 <= Lk <= CROSS_LK and 0 <= Lk2 <= CROSS_LK2
-            and lib().fyc_tcgen05_available() == 1)
+def cross_attention_tc_ok(dtype, D, Lk, Lk2, impl=None):
+    return use_cross_tc and D in (40, 64, 80) and 1 <= Lk <= CROSS_LK and 0 <= Lk2 <= CROSS_LK2 and _tc_open(dtype, impl)
 
 
 def cross_dkp(D):

@@ -671,7 +671,7 @@ class UNet3DConditionModel(ParamTreeModel):
         conv runs on the tensor cores, else the model's true input channels."""
         w = self._p("conv_in.weight")
         cin = w.shape[1]
-        if self._compute_dtype in ops.HALF_DTYPES and cin % 8 != 0 and cin <= 16 and ops.tc_ok(self._compute_dtype, 1 << 20):
+        if cin % 8 != 0 and cin <= 16 and ops.tc_ok(self._compute_dtype, 1 << 20):
             return 16
         return cin
 

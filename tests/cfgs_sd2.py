@@ -1,5 +1,5 @@
-"""Test configuration of the SD-2.x-based motion model ("mini" = the reference architecture at reduced width / depth), and the two
-adapters its tests need around the shared test infrastructure.
+"""Test configuration of the SD-2.x-based motion model ("mini" = the reference architecture at reduced width / depth), and the state-dict
+adapter its oracle needs.
 
 The mini model keeps the unet_additional_kwargs of configs/training/org_config_files/training_14M_448x256_w_multi_scale_w_fps_sd_v2.1.yaml on
 the SD-2.1 unet/config.json settings (use_linear_projection, upcast_attention, per-level attention_head_dim, 1024-wide text context),
@@ -11,9 +11,7 @@ import re
 
 import torch
 
-from followyourclick_b200 import _lib, ops
 from oracle.ref_unet import default_unet_config
-from tests import ops_emulator
 
 SD2_CTX_DIM = 1024
 _MM_SD2 = dict(num_attention_heads=4, num_transformer_block=1, attention_block_types=("Temporal_Self", "Temporal_Self"),
@@ -54,20 +52,3 @@ def oracle_state_dict(sd):
     270-295); the oracle applies them as 1x1 convolutions, which is the same per-token product y = W x + b.  The Linear weight [C, C] is
     that convolution's [C, C, 1, 1] filter; nothing else differs."""
     return {k: (v.reshape(*v.shape, 1, 1) if v.dim() == 2 and _SPATIAL_PROJ.search(k) else v) for k, v in sd.items()}
-
-
-def _self_attention_tc_ok(dtype, L, D):
-    return (ops_emulator.TC_EMULATED and ops._impl != _lib.IMPL_SIMT and dtype == torch.bfloat16 and D in (40, 64) and L % 128 == 0)
-
-
-def _cross_attention_tc_ok(dtype, D, Lk, Lk2):
-    return (ops_emulator.TC_EMULATED and ops.use_cross_tc and ops._impl != _lib.IMPL_SIMT and dtype == torch.bfloat16 and D in (40, 64, 80)
-            and 1 <= Lk <= ops.CROSS_LK and 0 <= Lk2 <= ops.CROSS_LK2)
-
-
-def install_emulator(monkeypatch):
-    """tests/ops_emulator.install, with the two tensor-core eligibility predicates mirroring the library's current ones (head dim 64
-    admitted): the emulated entry points themselves already serve D = 64 (64-column q / k heads, packed keys with head stride 64)."""
-    ops_emulator.install(monkeypatch)
-    monkeypatch.setattr(ops, "self_attention_tc_ok", _self_attention_tc_ok)
-    monkeypatch.setattr(ops, "cross_attention_tc_ok", _cross_attention_tc_ok)

@@ -652,7 +652,7 @@ def gemm_case(dtype, M, N, K, device, bias=True, residual=False, rpg=0, alpha=1.
     impl_code = {None: None, "simt": _lib.IMPL_SIMT}[impl]
 
     # the unfused GEGLU (CUDA-core path) writes packed rows: its output view is contiguous inside guard bands
-    fused = geglu and ops.tc_ok(dtype, M) and impl is None
+    fused = geglu and ops.tc_ok(dtype, M, impl_code)
     ldo = None if geglu and not fused else n_out + PAD
 
     def call(v, alloc):

@@ -5,9 +5,11 @@ classes on CPU - weight packing (fused q/k/v, 64-padded heads, GEGLU interleave,
 padded heads), the ClipContext hoisting, the Resampler, the pipeline plumbing - the CPU tests swap ``ops`` for this module's
 functions, which restate each kernel's *documented contract* (include/fyc.h) with torch ops in fp32 and round to the storage
 dtype exactly once, like the kernels do.  The host code under test is the product's own; only the kernel launches are replaced.
-Nothing in ``followyourclick_b200/`` imports this file, and it is never used on a GPU box (the ``-m gpu`` tests call the real
-library through the C ABI).
+The route rules that pick a kernel (ops.tc_ok, ops.self_attention_tc_ok, ...) are the product's too: the emulator answers only
+the hardware query under them, ops.tc_available, with True.  Nothing in ``followyourclick_b200/`` imports this file, and it is
+never used on a GPU box (the ``-m gpu`` tests call the real library through the C ABI).
 """
+import inspect
 import math
 
 import torch
@@ -15,23 +17,19 @@ import torch.nn.functional as F
 
 from followyourclick_b200 import _lib, ops
 
-TC_EMULATED = True        # report the tensor-core path as available for bf16, so its packing / layout branches are the ones exercised
-
 
 def _store(y, dtype):
     return y.to(dtype)
 
 
-def tc_ok(dtype, M):
-    return TC_EMULATED and ops._impl != _lib.IMPL_SIMT and dtype == torch.bfloat16 and M >= 64
+def tc_available():
+    """the tensor cores are reported available, so the route rules of ops send 16-bit calls down the tensor-core paths and the host
+    code's packing / layout branches for them are the ones exercised"""
+    return True
 
 
 def require_cuda(t, what):
     return None
-
-
-def ln_fold_ok(dtype, M, C):
-    return ops.use_ln_fold and tc_ok(dtype, M) and C % 8 == 0 and C <= 2048
 
 
 def layernorm_stats(x, eps=1e-5):
@@ -43,7 +41,7 @@ def layernorm_stats(x, eps=1e-5):
 
 def gemm(A, W, bias=None, residual=None, rowbias=None, rows_per_group=0, alpha=1.0, geglu=False, out_f32=False, out=None, impl=None, ln=None, A2=None):
     if ln is not None:          # fyc.h FYC_EPI_LNFOLD: row-centred weights, the epilogue scales the accumulator by rstd
-        assert A2 is None and alpha == 1.0 and residual is None and not out_f32 and tc_ok(A.dtype, A.shape[0])
+        assert A2 is None and alpha == 1.0 and residual is None and not out_f32 and ops.tc_ok(A.dtype, A.shape[0], impl)
     if A2 is not None:          # fyc.h A2: the K dimension is the concatenation [A | A2]
         A = torch.cat([A, A2], dim=-1)
     y = alpha * (A.float() @ W.float().transpose(-1, -2))
@@ -90,8 +88,7 @@ def conv3x3(x, w, bias=None, residual=None, rowbias=None, images_per_group=0, st
             pad_mode=0, w_phases=None):
     assert x.is_contiguous() and w.is_contiguous() and x.dtype == w.dtype
     NB, H, W_, Cin = x.shape
-    if upsample == 2 and w_phases is not None and ops.use_up2_phases and tc_ok(x.dtype, NB * H * W_) and residual is None \
-            and rowbias is None and not out_f32:
+    if upsample == 2 and w_phases is not None and ops.up2_phases_ok(x.dtype, NB * H * W_, residual, rowbias, out_f32, impl):
         assert tuple(w_phases.shape) == (4, w.shape[0], 2, 2, Cin) and w_phases.dtype == x.dtype
         return _store(_phase_conv(x, w_phases, bias), x.dtype).contiguous()
     xr = x.float().permute(0, 3, 1, 2)
@@ -162,10 +159,6 @@ def transpose_tokens(x, col0, C):
     return x[:, :, col0:col0 + C].transpose(1, 2).contiguous()
 
 
-def self_attention_tc_ok(dtype, L, D):
-    return TC_EMULATED and ops._impl != _lib.IMPL_SIMT and dtype == torch.bfloat16 and D == 40 and L % 128 == 0
-
-
 def self_attention_tc(qk, q_col0, k_col0, vt, heads, D, scale):
     NB, L, _ = qk.shape
     q = qk[:, :, q_col0:q_col0 + heads * 64].float().reshape(NB, L, heads, 64).transpose(1, 2)
@@ -173,10 +166,6 @@ def self_attention_tc(qk, q_col0, k_col0, vt, heads, D, scale):
     v = vt.float().reshape(NB, heads, D, L).transpose(2, 3)
     p = torch.softmax(q @ k.transpose(-1, -2) * scale, dim=-1)
     return _store((p @ v).transpose(1, 2).reshape(NB, L, heads * D), qk.dtype)
-
-
-def self_attention_tc80_ok(dtype, L, D):
-    return TC_EMULATED and ops.use_attn_d80 and ops._impl != _lib.IMPL_SIMT and dtype == torch.bfloat16 and D == 80 and L % 256 == 0
 
 
 def self_attention_tc_d80(qkv, q_col0, k_col0, vt, heads, scale):
@@ -187,11 +176,6 @@ def self_attention_tc_d80(qkv, q_col0, k_col0, vt, heads, scale):
     v = vt.float().reshape(NB, heads, D, L).transpose(2, 3)
     p = torch.softmax(q @ k.transpose(-1, -2) * scale, dim=-1)
     return _store((p @ v).transpose(1, 2).reshape(NB, L, heads * D), qkv.dtype)
-
-
-def cross_attention_tc_ok(dtype, D, Lk, Lk2):
-    return (TC_EMULATED and ops.use_cross_tc and ops._impl != _lib.IMPL_SIMT and dtype == torch.bfloat16 and D in (40, 80)
-            and 1 <= Lk <= ops.CROSS_LK and 0 <= Lk2 <= ops.CROSS_LK2)
 
 
 def cross_attention_tc(q, k, vt, heads, D, scale, Lk, out, k2=None, vt2=None, Lk2=0, out_alpha=1.0, alpha2=1.0, kv_batch_div=1):
@@ -277,6 +261,28 @@ def build_unet_input(latents, mask, first, dup, dtype, c_pad=None, out=None):
     return x
 
 
+def build_unet_input_first(latents, first, dup, dtype, mode, c_pad=None, out=None):
+    b, c, f, h, w = latents.shape
+    cin = 8 if mode & ops.FIRST_CONCAT else 4
+    c_pad = cin if c_pad is None else c_pad
+    if mode & ops.FIRST_FRAME:
+        latents[:, :, 0] = first                      # in place: the DDIM step that follows reads the replaced frame
+    x = torch.zeros(b, f, h, w, c_pad)
+    x[..., :4] = latents.permute(0, 2, 3, 4, 1)
+    if mode & ops.FIRST_CONCAT:
+        x[..., 4:8] = first.permute(0, 2, 3, 1)[:, None]
+    x = _store(torch.cat([x] * dup, dim=0), dtype)
+    if out is not None:
+        out.copy_(x)
+        return out
+    return x
+
+
+def first_frame_temb_rows(temb, B, F):
+    idx = torch.tensor([B if f == 0 else bi for bi in range(B) for f in range(F)])
+    return temb[idx].contiguous()
+
+
 def cfg_ddim_step(pred, sample, coefs, noise=None, out=None, single=None, video_scale=0.0):
     c = coefs
     n = sample.numel()
@@ -318,13 +324,24 @@ def video_grid_u8(video, nrow=6, padding=2, rescale=False):
     return torch.from_numpy(np.stack(ref_util.video_frames_uint8(video, rescale=rescale, n_rows=nrow)))
 
 
-_NAMES = ["tc_ok", "require_cuda", "ln_fold_ok", "layernorm_stats", "gemm", "conv3x3", "groupnorm", "layernorm", "attention", "transpose_tokens", "self_attention_tc_ok",
-          "self_attention_tc", "self_attention_tc80_ok", "self_attention_tc_d80", "cross_attention_tc_ok", "cross_attention_tc", "temporal_attention", "softmax_rows", "timestep_embed", "silu", "gelu", "upsample_nearest2x",
-          "concat_channels", "ncfhw_to_nfhwc", "nfhwc_to_ncfhw", "build_unet_input", "cfg_ddim_step", "frames_finalize", "video_grid_u8"]
+_NAMES = ["tc_available", "require_cuda", "layernorm_stats", "gemm", "conv3x3", "groupnorm", "layernorm", "attention", "transpose_tokens",
+          "self_attention_tc", "self_attention_tc_d80", "cross_attention_tc", "temporal_attention", "softmax_rows", "timestep_embed", "silu", "gelu",
+          "upsample_nearest2x", "concat_channels", "ncfhw_to_nfhwc", "nfhwc_to_ncfhw", "build_unet_input", "build_unet_input_first",
+          "first_frame_temb_rows", "cfg_ddim_step", "frames_finalize", "video_grid_u8"]
+
+
+def _library_callers():
+    """the public functions of ops whose own code calls into the library: they name ``lib`` (a query or launch) or ``check`` (the status
+    of a launch, also of those made through a private helper such as ops._tc_entry)"""
+    return {n for n, f in vars(ops).items() if inspect.isfunction(f) and f.__module__ == ops.__name__ and not n.startswith("_")
+            and {"lib", "check"} & set(f.__code__.co_names)}
 
 
 def install(monkeypatch):
-    """Replace every kernel-launching function of followyourclick_b200.ops for the duration of a test."""
+    """Replace the hardware query ops.tc_available (answered True), ops.require_cuda and every kernel-launching function of
+    followyourclick_b200.ops for the duration of a test.  The route rules (ops.tc_ok, ops.self_attention_tc_ok, ...) stay the product's."""
+    missing = _library_callers() - set(_NAMES)
+    assert not missing, f"ops functions that call the library have no emulation here: {sorted(missing)}"
     g = globals()
     for n in _NAMES:
         assert hasattr(ops, n), n

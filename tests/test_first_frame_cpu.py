@@ -1,7 +1,7 @@
 """CPU: the first-frame-conditioned motion models (use_first_frame_condition, use_first_frame_condition_concat).
 
   - the oracle reproduces the fixtures the unmodified reference wrote (tests/golden/make_golden_first_frame.py);
-  - the host code of UNet3DConditionModel / AnimationPipeline, with every kernel launch replaced by tests/ops_emulator_first_frame.py, reproduces them
+  - the host code of UNet3DConditionModel / AnimationPipeline, with every kernel launch replaced by tests/ops_emulator.py, reproduces them
     (mini UNet and 2-step pipeline, both modes, shared CFG prefix on and off, CUDA-graph bookkeeping and the eager loop);
   - every combination the reference cannot sample raises, naming both options.
 Tolerances are the engine's own (tests/test_engine_gpu.py): fp32 rel-L2 <= 1e-4, bf16 rel-L2 <= 3e-2, video max-abs <= 2e-3 (fp32) /
@@ -13,7 +13,7 @@ import os
 import pytest
 import torch
 
-from tests import ops_emulator_first_frame
+from tests import ops_emulator
 from tests.cfgs_first_frame import PIPE_CASES, UNET_CASES
 
 GOLD = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
@@ -22,7 +22,7 @@ DTYPES = [(torch.float32, 1e-4), (torch.bfloat16, 3e-2)]
 
 @pytest.fixture
 def emulated(monkeypatch):
-    ops_emulator_first_frame.install(monkeypatch)
+    ops_emulator.install(monkeypatch)
     torch.set_num_threads(8)
 
 

@@ -1,6 +1,6 @@
 """CPU: the opt-in fp16 tensor-core mode - C ABI constant, the compute-dtype API, the fp16 LN-folded weights, and the host logic of the
-UNet / VAE / pipeline in fp16 with every kernel launch emulated (tests/ops_emulator.py, with the adapter below admitting fp16 on the
-tensor-core routes exactly as followyourclick_b200.ops now does).  The real fp16 kernels are checked by tests/test_fp16_gpu.py.
+UNet / VAE / pipeline in fp16 with every kernel launch emulated (tests/ops_emulator.py; the tensor-core routes are the ones the rules of
+followyourclick_b200.ops pick for fp16).  The real fp16 kernels are checked by tests/test_fp16_gpu.py.
 """
 import os
 import re
@@ -13,42 +13,11 @@ from tests import ops_emulator
 from tests.fp16_helpers import literal_fp16_to
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-HALF = (torch.bfloat16, torch.float16)
-
-
-# ---- emulator adapter: the tensor-core eligibility predicates of ops, 16-bit set {bf16, fp16} ---------------------------------------
-def _tc_ok(dtype, M):
-    return ops_emulator.TC_EMULATED and ops._impl != _lib.IMPL_SIMT and dtype in HALF and M >= 64
-
-
-def _ln_fold_ok(dtype, M, C):
-    return ops.use_ln_fold and _tc_ok(dtype, M) and C % 8 == 0 and C <= 2048
-
-
-def _self_attention_tc_ok(dtype, L, D):
-    return ops_emulator.TC_EMULATED and ops._impl != _lib.IMPL_SIMT and dtype in HALF and D in (40, 64) and L % 128 == 0
-
-
-def _self_attention_tc80_ok(dtype, L, D):
-    return ops_emulator.TC_EMULATED and ops.use_attn_d80 and ops._impl != _lib.IMPL_SIMT and dtype in HALF and D == 80 and L % 256 == 0
-
-
-def _cross_attention_tc_ok(dtype, D, Lk, Lk2):
-    return (ops_emulator.TC_EMULATED and ops.use_cross_tc and ops._impl != _lib.IMPL_SIMT and dtype in HALF and D in (40, 64, 80)
-            and 1 <= Lk <= ops.CROSS_LK and 0 <= Lk2 <= ops.CROSS_LK2)
-
-
-def install_emulator(monkeypatch):
-    ops_emulator.install(monkeypatch)
-    for name, fn in (("tc_ok", _tc_ok), ("ln_fold_ok", _ln_fold_ok), ("self_attention_tc_ok", _self_attention_tc_ok),
-                     ("self_attention_tc80_ok", _self_attention_tc80_ok), ("cross_attention_tc_ok", _cross_attention_tc_ok)):
-        monkeypatch.setattr(ops, name, fn)
-    monkeypatch.setattr(ops_emulator, "tc_ok", _tc_ok)       # the emulated gemm / conv3x3 ask it which path they stand for
 
 
 @pytest.fixture
 def emulated(monkeypatch):
-    install_emulator(monkeypatch)
+    ops_emulator.install(monkeypatch)
     literal_fp16_to(monkeypatch)
     torch.set_num_threads(8)
     yield

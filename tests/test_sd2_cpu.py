@@ -1,7 +1,6 @@
 """CPU: SD-2.x-based motion models (linear transformer projections, upcast attention, per-level heads of head dim 64, 1024-wide text
 context) - the oracle against the unmodified reference's SD-2 fixtures, the engine's key contract and checkpoint loading, and the engine's
-host logic with every kernel launch emulated (tests/ops_emulator.py via tests/cfgs_sd2.install_emulator), including which attention
-entry points the bf16 mode routes to.
+host logic with every kernel launch emulated (tests/ops_emulator.py), including which attention entry points the bf16 mode routes to.
 
 Tolerances are those of the SD-1.5 host-logic tests (tests/test_host_emulated_cpu.py): fp32 rel-L2 <= 1e-4, bf16 rel-L2 <= 3e-2, pipeline
 video max-abs <= 2e-3 (fp32) / PSNR >= 30 dB (bf16).
@@ -12,7 +11,8 @@ import os
 import pytest
 import torch
 
-from tests.cfgs_sd2 import MINI_SD2, MINI_SD2_2D, install_emulator, mini_sd2_oracle_cfg, oracle_state_dict, sd2_inputs
+from tests import ops_emulator
+from tests.cfgs_sd2 import MINI_SD2, MINI_SD2_2D, mini_sd2_oracle_cfg, oracle_state_dict, sd2_inputs
 from tests.sd2_helpers import (make_sd2_unet, run_sd2_pipeline_case, run_sd2_unet2d_case, run_sd2_unet_case, sd2_keys, sd2_pins)
 
 DTYPES = [(torch.float32, 1e-4), (torch.bfloat16, 3e-2)]
@@ -114,7 +114,7 @@ def test_from_pretrained_2d_loads_an_sd21_unet_folder(tmp_path, capsys):
 # ------------------------------------------------------------------------------------------------ (d) host logic, kernels emulated
 @pytest.fixture
 def emulated(monkeypatch):
-    install_emulator(monkeypatch)
+    ops_emulator.install(monkeypatch)
     torch.set_num_threads(8)
     yield monkeypatch
 
